@@ -62,7 +62,7 @@ WORKLOADS = {
 # the BASELINE.json configs next to the headline (config 2), in the `configs` array of the default run
 EXTRA_CONFIGS = [("3: Hand + 92 touch sensors", "hand_block_touch"), ("4: AntMaze_Large, 1024 envs/GPU (8192 over 8 GPUs)", "antmaze_large"),
                  ("5a: AdroitHandHammer", "adroit_hammer"), ("5b: FrankaKitchen", "franka_kitchen")]
-FP32_PEAK_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12   # non-tensor FP32: 148 SMs x 128 lanes x 2 (FMA) x 1.965 GHz = 74.4
+FP32_PEAK_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12   # non-tensor FP32 of an H100 SXM: 132 SMs x 128 lanes x 2 (FMA) x 1.98 GHz = 66.9
 
 
 def measured_peaks():
@@ -70,7 +70,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -213,7 +213,7 @@ class Harness:
         if self.world > 1:
             os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
             dist.init_process_group("nccl", device_id=self.dev)
-        self.flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=self.dev)  # > L2 (126 MB)
+        self.flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=self.dev)  # > L2 (50 MB on an H100)
 
     def barrier(self):
         if self.world > 1:
@@ -249,10 +249,13 @@ def make_env(H, workload, n, rng_mode):
     return env
 
 
-def time_workload(H, workload, n, steps, warmup, rng_mode="torch", nvtx=False, sample_clocks=False, gather=False):
+def time_workload(H, workload, n, steps, warmup, rng_mode="torch", nvtx=False, sample_clocks=False, gather=False, keep_last=False):
     """Three timed arms over the same env: (1) `value`: CUDA events around env.step with device-resident actions, (2) the step
     kernel alone, (3) end to end with HOST buffers -- pinned actions H2D, the packed result rows D2H, every step.  All times are
-    per-rank sums; the caller takes the max over ranks."""
+    per-rank sums; the caller takes the max over ranks.  keep_last: also return what the last step of arm (1) handed its caller
+    (`outputs`: name -> numpy array)."""
+    import numpy as np
+
     torch = H.torch
     env_id, nact, nsub, b_alg, _ = WORKLOADS[workload]
     env = make_env(H, workload, n, rng_mode)
@@ -271,15 +274,20 @@ def time_workload(H, workload, n, steps, warmup, rng_mode="torch", nvtx=False, s
     kev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     nv = torch.cuda.nvtx if nvtx else None   # --nvtx: ranges for ncu --nvtx filtering (SURVEY.md section 5, tracing)
     reset_masks = []
+    last = None
     for k in range(steps):
         flush.fill_(float(k))  # evict L2 between timed iterations (outside the timed interval)
         ev[k][0].record()
         if nv:
             nv.range_push(f"env.step {k}")
-        _, _, _, _, info = env.step(tape[k % 64])
+        o, r, te, tr, info = env.step(tape[k % 64])
         if nv:
             nv.range_pop()
         ev[k][1].record()
+        if keep_last and k == steps - 1:
+            # copied here: the later arms step the same env and reuse its output buffers
+            last = {**(dict(o) if isinstance(o, dict) else {"observation": o}), "reward": r, "terminated": te, "truncated": tr}
+            last = {key: v.detach().cpu().numpy().astype(np.float64 if v.dtype == torch.float64 else np.float32) for key, v in last.items()}
         if "_final_obs" in info:
             reset_masks.append(info["_final_obs"])   # same-step autoreset happened inside this timed step
     H.barrier()
@@ -359,7 +367,7 @@ def time_workload(H, workload, n, steps, warmup, rng_mode="torch", nvtx=False, s
     res = dict(workload=workload, env_id=env_id, n=n, nsub=nsub, nact=nact, b_alg=b_alg, ms=ms, kms=kms, e2e_ms=e2e_s * 1e3,
                e2e_gather_ms=None if e2e_gather_s is None else e2e_gather_s * 1e3, launches=launches, resets=resets, h2d=h2d, d2h=d2h,
                clocks=clocks, overflow_env_steps=int(env.backend.overflow_counter[0]),
-               wpb=None, gathered_rows=None if gatherer is None else int(gatherer.rows))
+               wpb=None, gathered_rows=None if gatherer is None else int(gatherer.rows), outputs=last)
     env.close()
     return res
 
@@ -390,6 +398,26 @@ def roofline_object(res, steps):
     return roof
 
 
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(outputs, out_dir, suffix=""):
+    """--dump-outputs: one DIR/<name>.npy per array of the last timed step.  Above 64 MB in all, the same fixed, seeded sample of
+    envs is kept from every array and its env indices are written as `env_index.npy`."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(outputs["reward"])
+    total = sum(a.nbytes for a in outputs.values())
+    if total > DUMP_LIMIT_BYTES:
+        keep = max(1, DUMP_LIMIT_BYTES // (total // n + 8))   # + 8 bytes per kept env for its index
+        rows = np.sort(np.random.default_rng(0).choice(n, size=keep, replace=False))
+        outputs = {k: a[rows] for k, a in outputs.items()}
+        outputs["env_index"] = rows.astype(np.float64)
+    for k, a in outputs.items():
+        np.save(os.path.join(out_dir, f"{k}{suffix}.npy"), a)
+
+
 def run_ours(args):
     H = Harness()
     world, rank = H.world, H.rank
@@ -406,7 +434,10 @@ def run_ours(args):
         headline = mixed[rank]
         args.envs_per_gpu = args.envs_per_gpu or 1024
     n = args.envs_per_gpu or WORKLOADS[headline][4]
-    res = time_workload(H, headline, n, args.steps, args.warmup, rng_mode=args.rng_mode, nvtx=args.nvtx, sample_clocks=True, gather=args.gather)
+    res = time_workload(H, headline, n, args.steps, args.warmup, rng_mode=args.rng_mode, nvtx=args.nvtx, sample_clocks=True, gather=args.gather,
+                        keep_last=args.dump_outputs is not None)
+    if args.dump_outputs is not None:
+        dump_outputs(res["outputs"], args.dump_outputs, f"_rank{rank}" if world > 1 else "")
     if os.environ.get("B200SIM_BENCH_DEBUG"):
         print(f"[rank {rank}] ms/step {res['ms'] / args.steps:.3f} kernel {res['kms']:.3f} e2e {res['e2e_ms'] / args.steps:.3f}", file=sys.stderr)
     ms, e2e_ms, kms, e2e_g = H.max_over_ranks([res["ms"], res["e2e_ms"], res["kms"], res["e2e_gather_ms"] or 0.0])
@@ -489,6 +520,8 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the `configs` array (the other BASELINE configs)")
     ap.add_argument("--config-steps", type=int, default=20, help="timed steps of each entry of the `configs` array")
     ap.add_argument("--gather", action="store_true", help="N > 1: also time e2e with the NCCL all-gather of the packed rows")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of the headline workload returned as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--nvtx", action="store_true", help="NVTX range around every timed env.step (profiling runs only)")
     ap.add_argument("--rng-mode", default="torch", choices=["torch", "device"],
                     help="reset draws of the Fetch workload: torch's device generator (default) or in-kernel (b200sim_reset)")

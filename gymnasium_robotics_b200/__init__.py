@@ -1,4 +1,4 @@
-"""gymnasium_robotics_b200: B200-native batched simulator behind the Gymnasium-Robotics env API (hot path only).
+"""gymnasium_robotics_b200: batched CUDA simulator (H100, sm_90a) behind the Gymnasium-Robotics env API (hot path only).
 
 Drop-in boundary mirrored from the reference registry (gymnasium_robotics/__init__.py:12-80): the same env ids and
 kwargs, constructed as batched vector envs.  `make_vec(id, num_envs=N)` works without gymnasium; when gymnasium is
@@ -60,7 +60,7 @@ for _rt, _suffix in (("dense", ""), ("sparse", "Sparse")):
 def make_vec(env_id: str, num_envs: int = 1, **kwargs):
     """Batched replacement for `gym.make_vec(env_id, num_envs=...)` (reference ids, e.g. "FetchPickAndPlace-v4")."""
     if env_id.startswith("FrankaKitchen"):
-        # kernel build csrc/b200sim_kitchen*.cu (joint-equality rows, condim 6, two-level broad phase); validated on a B200 against
+        # kernel build csrc/b200sim_kitchen*.cu (joint-equality rows, condim 6, two-level broad phase); validated on the GPU against
         # the oracle env and the host emulation (tests/test_zz_kitchen_gpu.py)
         if env_id != "FrankaKitchen-v1":
             raise KeyError(f"{env_id!r}: the reference registers FrankaKitchen-v1 only")

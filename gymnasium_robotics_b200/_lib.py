@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200SIM_LIB") or os.path.join(_HERE, "libb200sim.so")
 _LIB = None
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DB200_BLOCK_ALIGN", "-DB200_CHOL_SMEM",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DB200_BLOCK_ALIGN", "-DB200_CHOL_SMEM",
               "-prec-div=false", "-prec-sqrt=false"] + \
     os.environ.get("B200SIM_NVCC_EXTRA", "").split()
 
@@ -66,7 +66,7 @@ class KeepC(ctypes.Structure):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """nvcc-compile csrc/b200sim.cu and csrc/b200sim_wide.cu for sm_100a into the in-tree libb200sim.so (cross-compiles
+    """nvcc-compile csrc/b200sim.cu and csrc/b200sim_wide.cu for sm_90a into the in-tree libb200sim.so (cross-compiles
     without a GPU; the two translation units are compiled in parallel)."""
     names = ("b200sim", "b200sim_wide", "b200sim_kitchen", "b200sim_kitchen_groups", "b200sim_kitchen_hull")
     srcs = [os.path.join(_HERE, "csrc", n + ".cu") for n in names]
@@ -80,7 +80,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
     rcs = [p.wait() for p in procs]
     if any(rcs):
         raise subprocess.CalledProcessError(max(rcs), "nvcc -c (b200sim)")
-    subprocess.check_call(["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs)
+    subprocess.check_call(["nvcc", "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs)
     for o in objs:
         os.remove(o)
     return LIB_PATH

@@ -1,4 +1,4 @@
-// b200sim: CUDA kernels (sm_100a) + the C-ABI of include/b200sim.h.
+// b200sim: CUDA kernels (sm_90a) + the C-ABI of include/b200sim.h.
 //
 // One warp integrates one env for a whole env-step (all sub-steps on chip); WPB warps share one copy of the model
 // constants that a single thread stages into shared memory with a TMA bulk copy (cp.async.bulk + mbarrier).
@@ -13,8 +13,7 @@
 #include "step_kernel.cuh"
 #include "reset_sample.cuh"
 
-// warps (= envs) per block: 28 fills an SM in one wave at 4096 envs per GPU; smaller batches use smaller blocks so
-// that every SM still gets work (e.g. the 1024-env shards of BASELINE config 4)
+// warps (= envs) per block: at most 28 (the shared memory of one block); b200sim_create picks the size from the SM count
 #define B200_WPB_MAX 28
 
 #ifdef B200_STAGE_TIMING
@@ -116,7 +115,7 @@ __global__ void reach_reset_kernel(b200sim_reach_reset_t p, unsigned long long s
 
 // ---------------------------------------------------------------------------------------------------------------
 #define B200_FOR_ALL_VARIANTS(X) X(7, 14) X(7, 15) X(7, 21) X(14, 14) X(14, 15) X(14, 21) X(28, 14) X(28, 15) X(28, 21) \
-  X(7, 22) X(14, 22) X(28, 22) X(7, 30) X(14, 30)
+  X(7, 22) X(14, 22) X(28, 22) X(7, 30) X(14, 30) X(8, 14) X(8, 15) X(8, 21) X(8, 22) X(16, 14) X(16, 15) X(16, 21) X(16, 22)
 
 // wide build (models with 33..40 dofs), compiled from b200sim_wide.cu with 64-bit dof masks
 extern "C" int b200sim_wide_setattr(int wpb, int smem_bytes);
@@ -288,40 +287,46 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   t.st_stride = (o + 3) & ~3;
   DevGuard guard(device);
   if (!guard.ok) { delete h; return fail(nullptr, "b200sim_create: cudaSetDevice failed", -7); }
-  int nsm = 148;
+  int nsm = 132;
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device);
-  h->wpb = (num_envs + nsm - 1) / nsm <= 7 ? 7 : ((num_envs + nsm - 1) / nsm <= 14 ? 14 : 28);
   h->nvp = dh->nv <= 14 ? 14 : (dh->nv == 15 ? 15 : (dh->nv <= 21 ? 21 : (dh->nv <= 30 ? 30 : (dh->nv > 32 && dh->nv <= B200_WIDE_NVP ? B200_WIDE_NVP : 0))));  // smallest built size >= nv (identity padding)
   if (h->nvp == 0) { delete h; return fail(nullptr, "b200sim_create: no kernel instantiation for this nv (31, 32 or > 36)", -8); }
   if ((t.kind == TASK_HAND || t.kind == TASK_HAND_REACH || TASK_IS_ADROIT(t.kind)) && h->nvp < 30) h->nvp = 30;  // the hand task code is compiled into this build only
   if (dh->nv <= 21 && dh->any_convex_pair) h->nvp = 22;  // arm build that carries the general convex collider (FetchSlide's puck)
   if (dh->nv <= 21 && (dh->nten > 0 || dh->nfric > 0 || dh->nsensor > 0 || dh->any_round_pair)) h->nvp = 30;  // hand features live in the NVP = 30 build
-  if (h->nvp == 30 && h->wpb > 14) h->wpb = 14;  // the large models' scratch does not fit 28 envs per block
   auto fits = [&](int w) { return ((size_t)dh->hot_words + (size_t)w * dh->scr_words) * 4 + 64 <= 232448; };
+  auto built = [&](int w) {   // an instantiation <w, nvp> exists (the wide ones: b200sim_wide.cu)
+    if (h->nvp == B200_WIDE_NVP) return w == 7 || w == 10 || w == 13 || w == 14;
+    bool b = false;
+#define B200_HAS(W, V) b = b || (w == W && h->nvp == V);
+    B200_FOR_ALL_VARIANTS(B200_HAS)
+#undef B200_HAS
+    return b;
+  };
   const char* ov = getenv("B200SIM_WPB");   // experiments: a block size that has no instantiation for this build is an error, not a no-op
   const int ovw = ov ? atoi(ov) : 0;
   if (h->kitchen) {
     if (dh->nv > 31) { delete h; return fail(nullptr, "b200sim_create: the kitchen build is instantiated for nv <= 31", -8); }
     h->nvp = B200_KITCHEN_NVP;
-    h->wpb = h->wpb <= 7 ? 7 : ((h->kitchen_groups && fits(11)) ? 11 : (fits(10) ? 10 : 7));
+    h->wpb = (num_envs + nsm - 1) / nsm <= 7 ? 7 : ((h->kitchen_groups && fits(11)) ? 11 : (fits(10) ? 10 : 7));
     if (ov) {
       if (!((ovw == 7 || ovw == 10 || (ovw == 11 && h->kitchen_groups)) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no kitchen kernel variant that fits", -8); }
       h->wpb = ovw;
     }
-  } else if (h->nvp == B200_WIDE_NVP) {
-    // wide build: the largest block of {14, 13, 10, 7} warps whose scratch fits the 227 KB of shared memory (14 envs of the
-    // 33-dof hammer model, 13 of the 36-dof relocate model), 7 for small batches so that every SM still gets a block
-    const int want = h->wpb, cands[4] = {14, 13, 10, 7};
-    h->wpb = 7;
-    for (int k = 3; k >= 0; k--)
-      if (cands[k] <= (want > 7 ? 14 : 7) && fits(cands[k])) h->wpb = cands[k];
+  } else {
+    // one block per SM (shared instruction cache), as few waves as the largest fitting block needs, and the smallest block that
+    // needs no more (fewer warps per SM finish sooner): 4096 envs on 132 SMs -> two waves of 16 warps, 1024 envs -> one wave of 8
+    auto waves = [&](int w) { return ((num_envs + w - 1) / w + nsm - 1) / nsm; };
+    int wmax = 0;
+    for (int w = 1; w <= B200_WPB_MAX; w++)
+      if (built(w) && fits(w)) wmax = w;
+    h->wpb = wmax > 0 ? wmax : 7;   // 7 when nothing fits: refused below
+    for (int w = wmax; w >= 1; w--)
+      if (built(w) && fits(w) && waves(w) == waves(wmax)) h->wpb = w;
     if (ov) {
-      if (!((ovw == 7 || ovw == 10 || ovw == 13 || ovw == 14) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no wide kernel variant that fits", -8); }
+      if (!(built(ovw) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no kernel variant that fits", -8); }
       h->wpb = ovw;
     }
-  } else if (ov) {
-    if (!((ovw == 7 || ovw == 14 || (ovw == 28 && h->nvp != 30)) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no kernel variant that fits", -8); }
-    h->wpb = ovw;
   }
   if (!fits(h->wpb)) { delete h; return fail(nullptr, "b200sim_create: the per-env scratch of this model does not fit the shared memory of one block", -8); }
   h->smem_bytes = ((size_t)dh->hot_words + (size_t)h->wpb * dh->scr_words) * 4;

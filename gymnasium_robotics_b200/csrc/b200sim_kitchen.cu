@@ -5,7 +5,7 @@
 // is regrouped into bounding-volume groups there and scanned in two levels (sim_core.cuh `collision`, DESIGN.md 3).
 // b200sim_kitchen_groups.cu includes this file with B200_KITCHEN_GROUPS defined: the same build with the two-level broad phase
 // (dmodel.h / sim_core.cuh); its kernels and entry points carry the suffix _groups so that both builds live in one library and
-// `b200sim_create` can pick either (B200SIM_KITCHEN_GROUPS=1; the plain build is the one validated on a B200 so far).
+// `b200sim_create` can pick either (B200SIM_KITCHEN_GROUPS=1; both builds are validated against each other on the GPU).
 #define B200_KITCHEN 1
 #if defined(B200_HULL)
 #define fetch_kernel fetch_kernel_hull

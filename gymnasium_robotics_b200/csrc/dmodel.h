@@ -27,7 +27,7 @@
 // (name, words-per-element, kind) ; kind selects the element count.  HOT arrays are staged into shared memory by every
 // block; COLD arrays (per-pair contact parameters, read only when a contact is created) stay in global memory.
 // Kitchen build with the two-level broad phase (-DB200_KITCHEN_GROUPS on top of -DB200_KITCHEN; the plain kitchen build keeps the
-// flat scan that was validated on a B200): the flat pair list (3 708 entries, 44 KB) leaves shared memory -- it is only read for the pairs of the
+// flat scan, its bit-exact reference): the flat pair list (3 708 entries, 44 KB) leaves shared memory -- it is only read for the pairs of the
 // bounding-volume groups that survive the first broad-phase level -- and the group table (one bounding sphere on one body
 // against one anchor geom, a contiguous run of pairs) is staged instead.
 #ifdef B200_KITCHEN_GROUPS

@@ -1,4 +1,4 @@
-// b200sim physics core: one warp integrates one env.  Hand-written for sm_100a; the same source compiles on the
+// b200sim physics core: one warp integrates one env.  Hand-written for sm_90a; the same source compiles on the
 // host with WARP_W == 1 for the test-only emulation harness in tests/hostsim (never part of the product library).
 //
 // Replaces `mujoco.mj_step(model, data, nstep=n_substeps)` (reference: gymnasium_robotics/envs/robot_env.py:340-341)
@@ -87,7 +87,7 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #endif
 
-// Address-space hint for the narrow-phase lane slots.  Measured on a B200 (profiles/bisect_r2c.log): with the hint on the slot
+// Address-space hint for the narrow-phase lane slots.  Observed on the GPU: with the hint on the slot
 // reference inside collision() the kernel reads garbage addresses (compute-sanitizer: invalid __shared__ read in the NEXT broad
 // phase; the 32-lane host emulation under ASan / UBSan is clean, the same build without the hint is clean on the GPU) -- the
 // slot address is a per-lane select between two scratch regions and nvcc 12.9 mis-handles the assumption there.  collision()
@@ -578,9 +578,9 @@ HD void ref_kb(const Ctx& c, const float* solref, float dmax_in, float* K, float
 
 // ---------------------------------------------------------------------------------------------------------------
 // 5. collision (plane-box, box-box; same decision logic as oracle/oracle.c, fp32)
-// Result of one candidate pair (at most 4 contacts): 29 words on the lane's stack.  Measured on a B200 (profiles/variants_r2e.log):
+// Result of one candidate pair (at most 4 contacts): 29 words on the lane's stack.  A/B-timed when it was chosen:
 // keeping the result in a shared-memory slot forces the lanes to park it in 28 registers before the contact records -- which the
-// slots overlay -- are written, and that costs 0.48 ms of the 3.7 ms step in the 72-register build.  What does move to shared memory is
+// slots overlay -- are written, which was measurably slower in the 72-register build.  What does move to shared memory is
 // the box-box routine's working set (BoxScratch): it is dead when the routine returns, so no parking is needed, and with it the
 // stack frame -- whose size x 132 k threads is what the local-memory write-back traffic scales with -- shrinks.
 struct ContactOut { float pos[4][3]; float nrm[4][3]; float dist[4]; int cnt; };

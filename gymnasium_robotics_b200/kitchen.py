@@ -93,9 +93,9 @@ class KitchenVectorEnv(CtorPickle):
         self.model = model if model is not None else load_model("franka_kitchen_hull" if mesh_collision == "hull" else "franka_kitchen")
         m = self.model
         self.task = make_kitchen_task(m, frame_skip)
-        # broadphase="groups" (default): the kernel build with the two-level broad phase (csrc/b200sim_kitchen_groups.cu) -- on a B200
-        # it matches the flat-scan build (tests/test_zz_kitchen_gpu.py) and is 1.5x faster (8.6 vs 12.6 ms per 2048-env step,
-        # profiles/kitchen_diag_r2a_after_fix.log); "flat": one scan over all 3 708 pairs.  The library reads the choice from the
+        # broadphase="groups" (default): the kernel build with the two-level broad phase (csrc/b200sim_kitchen_groups.cu) -- it
+        # matches the flat-scan build bit for bit (tests/test_zz_kitchen_gpu.py) and tests far fewer pairs per sub-step; "flat": one
+        # scan over all 3 708 pairs.  The library reads the choice from the
         # environment when the handle is created.
         broadphase = kwargs.get("broadphase", "flat" if os.environ.get("B200SIM_KITCHEN_GROUPS", "1") in ("0",) else "groups")
         if broadphase not in ("flat", "groups"):

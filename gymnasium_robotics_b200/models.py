@@ -1,8 +1,8 @@
 """Compiled model store.
 
-The reference's MJCF/STL assets are not redistributed; `build_models()` compiles them (when the reference checkout is
-present, i.e. in the build container) into constant-table blobs under ``gymnasium_robotics_b200/models/`` which are
-what ships and what the GPU box loads (``/root/reference`` does not exist there).
+The reference's MJCF/STL assets are not redistributed; `build_models()` compiles them (when B200SIM_REFERENCE_ASSETS names the
+reference checkout's ``gymnasium_robotics/envs/assets``) into constant-table blobs under ``gymnasium_robotics_b200/models/``,
+which are committed: they are what ships and what the library loads.
 """
 from __future__ import annotations
 
@@ -12,7 +12,7 @@ from .mjcf import Model, compile_mjcf
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 MODEL_DIR = os.path.join(_HERE, "models")
-REFERENCE_ASSETS = os.environ.get("B200SIM_REFERENCE_ASSETS", "/root/reference/gymnasium_robotics/envs/assets")
+REFERENCE_ASSETS = os.environ.get("B200SIM_REFERENCE_ASSETS", "")
 
 # model name -> MJCF path relative to the reference's assets directory
 MODEL_SOURCES = {

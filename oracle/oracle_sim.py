@@ -8,7 +8,9 @@ from __future__ import annotations
 
 import ctypes
 import os
+import shutil
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -20,8 +22,8 @@ _NATIVE = False
 
 
 def use_native_build():
-    """bench.py's CPU arm only: build and load liboracle with `-O3 -march=native` for the box it runs on (the default -O2 build is
-    what the parity tests use and what travels between machines).  Must be called before the first `lib()`."""
+    """bench.py's CPU arm only: build and load liboracle with `-O3 -march=native` for the machine it runs on (the default -O2
+    build is what the parity tests use and what build() leaves in the tree).  Must be called before the first `lib()`."""
     global _NATIVE
     if _LIB is None:
         _NATIVE = True
@@ -29,33 +31,33 @@ def use_native_build():
 
 def build(force: bool = False) -> str:
     """Compile oracle.c -> oracle/_build/liboracle.so with gcc (idempotent)."""
-    name, flags = "liboracle.so", ["-O2"]
-    if _NATIVE:
-        import hashlib
-        import platform
-
-        cpu = ""
-        try:
-            cpu = next((l for l in open("/proc/cpuinfo") if l.startswith("model name")), "")
-        except OSError:
-            pass
-        name = "liboracle_native_" + hashlib.sha1((platform.machine() + cpu).encode()).hexdigest()[:10] + ".so"
-        flags = ["-O3", "-march=native"]
-    out = os.path.join(_HERE, "_build", name)
+    out = os.path.join(_HERE, "_build", "liboracle.so")
     src = os.path.join(_HERE, "oracle.c")
     hdr = os.path.join(_HERE, "..", "include", "b200sim_model.h")
     if force or not os.path.exists(out) or (os.path.exists(src) and os.path.getmtime(out) < max(os.path.getmtime(src), os.path.getmtime(hdr))):
         os.makedirs(os.path.dirname(out), exist_ok=True)
         tmp = f"{out}.{os.getpid()}.tmp"
-        subprocess.check_call(["gcc"] + flags + ["-fPIC", "-shared", "-o", tmp, src, "-lm"])
+        subprocess.check_call(["gcc", "-O2", "-fPIC", "-shared", "-o", tmp, src, "-lm"])
         os.replace(tmp, out)
     return out
+
+
+def _load_native():
+    """The -O3 -march=native build, compiled afresh (about 2 s) in a private mkdtemp directory (the tree may be read-only; a fixed
+    shared path could be planted by another user), removed once the library is mapped."""
+    d = tempfile.mkdtemp(prefix="b200sim-oracle-")
+    try:
+        out = os.path.join(d, "liboracle_native.so")
+        subprocess.check_call(["gcc", "-O3", "-march=native", "-fPIC", "-shared", "-o", out, os.path.join(_HERE, "oracle.c"), "-lm"])
+        return ctypes.CDLL(out)
+    finally:
+        shutil.rmtree(d, ignore_errors=True)
 
 
 def lib():
     global _LIB
     if _LIB is None:
-        L = ctypes.CDLL(build())
+        L = _load_native() if _NATIVE else ctypes.CDLL(build())
         L.oracle_create.restype = ctypes.c_void_p
         L.oracle_create.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
         for f in ("oracle_destroy", "oracle_reset_data", "oracle_forward"):

@@ -120,6 +120,30 @@ def test_fetch_slide_tracks_oracle():
             assert float(r[i]) == float(orr)
 
 
+def test_free_motion_parity_outlier_is_one_ulp_away():
+    """Step 0, env 7 of the free-motion phase of test_gpu_parity.py's FetchPickAndPlace step parity (fingers in contact): one ulp on
+    the injected wrist-flex angle moves the emulated finger velocity (obs 23) by 2.2e-5, the error the sm_90a build shows there."""
+    n = 8
+    env = mk("FetchPickAndPlace", n, rng_mode="numpy")
+    env.reset(seed=100)
+    oracles = [oracle_env_from_model("FetchPickAndPlace", env.model) for _ in range(n)]
+    for i, o in enumerate(oracles):
+        o.reset(seed=100 + i)
+    a = np.random.default_rng(7).uniform(-1, 1, (n, 4)).astype(np.float32)   # the parity test's first actions
+    inject_oracle_state(env, oracles)
+    base = env.backend.state.clone()
+    want = oracles[7].step(a[7].astype(np.float64))[0]["observation"]
+    o, *_ = env.step(a)
+    assert np.abs(o["observation"][7].double().numpy() - want).max() < 2e-7
+    slot = env.backend.layout["qpos"] + int(env.model.jnt_qposadr[env.model.joint_id("robot0:wrist_flex_joint")])
+    st = base.clone()
+    st[7, slot] = float(np.nextafter(np.float32(st[7, slot].item()), np.float32(-np.inf)))
+    env.backend.state.copy_(st)
+    o, *_ = env.step(a)
+    d = np.abs(o["observation"][7].double().numpy() - want)
+    assert int(d.argmax()) == 23 and 1e-5 < d.max() < 8e-5
+
+
 def test_timelimit_and_next_step_autoreset():
     env = mk("FetchReach", 2, rng_mode="numpy", max_episode_steps=3)
     env.reset(seed=0)

@@ -1,11 +1,15 @@
-"""MJCF -> constant tables: sizes, MuJoCo compile rules, blob round trip, committed blobs in sync with the sources."""
+"""MJCF -> constant tables: sizes, MuJoCo compile rules, blob round trip, the committed Fetch blob against numbers from its sources."""
+import json
 import os
 
 import numpy as np
 import pytest
 
 from gymnasium_robotics_b200.mjcf import Model, compile_mjcf
-from gymnasium_robotics_b200.models import MODEL_DIR, MODEL_OVERRIDES, MODEL_SOURCES, REFERENCE_ASSETS, load_model
+from gymnasium_robotics_b200.models import load_model
+
+# numbers taken from the reference's Fetch MJCF and from a fresh compile of it (tests/golden/make_fetch_fixture.py)
+FETCH = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "fetch_fixture.json")))
 
 
 def test_committed_blobs_load_and_have_expected_sizes():
@@ -25,23 +29,18 @@ def test_blob_round_trip_is_lossless():
     assert m.names == m2.names
 
 
-@pytest.mark.needs_reference
-def test_committed_blobs_match_a_fresh_compile():
-    for name, rel in MODEL_SOURCES.items():
-        fresh = compile_mjcf(os.path.join(REFERENCE_ASSETS, rel), overrides=MODEL_OVERRIDES.get(name)).to_blob()
-        assert open(os.path.join(MODEL_DIR, name + ".b200m"), "rb").read() == fresh, name
-
-
-@pytest.mark.needs_reference
 def test_fused_runtime_model_keeps_the_dynamics():
     """Fusing jointless bodies (MuJoCo `fusestatic`) must not change the mass matrix; collision filters follow MuJoCo."""
     from oracle.oracle_sim import OracleSim
 
-    m = compile_mjcf(os.path.join(REFERENCE_ASSETS, "fetch/pick_and_place.xml"))
+    m = load_model("fetch_pick_and_place")
     s = OracleSim(m)
     s.forward()
-    assert np.abs(s.M - m._full_arrays["M0"]).max() < 1e-10  # oracle CRB on the fused tree vs dense sum on the MJCF tree
-    assert m.nbody == 16 and len(m._full.bodies) == 33  # 33 MJCF bodies (world included) fuse into 16
+    M0 = np.zeros((m.nv, m.nv))
+    M0[np.triu_indices(m.nv)] = FETCH["M0_upper"]
+    M0 = M0 + np.triu(M0, 1).T
+    assert np.abs(s.M - M0).max() < 1e-10  # oracle CRB on the fused tree vs dense sum on the MJCF tree
+    assert m.nbody == 16  # the 33 MJCF bodies (world included) fuse into 16
     geoms = m.names["geom"]
     pairs = {(geoms[a], geoms[b]) for a, b in zip(m.pair_geom1, m.pair_geom2)}
     assert ("robot0:r_gripper_finger_link", "robot0:l_gripper_finger_link") not in pairs  # <exclude>
@@ -95,7 +94,6 @@ def _xml_subtree_masses(path):
     return out
 
 
-@pytest.mark.needs_reference
 def test_fetch_closed_form_totals():
     """Total robot mass, the composite inertia seen by the three base slides, and the gravity load on the torso lift joint of the
     Fetch model: XML numbers against the compiled blob, the oracle (C, fp64) and the kernel emulation (fp32)."""
@@ -103,7 +101,7 @@ def test_fetch_closed_form_totals():
     from tests.hostsim import HostSim
     from gymnasium_robotics_b200.fetch import REF_POINT, welded_eq_data
 
-    sub = _xml_subtree_masses(os.path.join(REFERENCE_ASSETS, "fetch", "robot.xml"))
+    sub = FETCH["subtree_mass"]
     robot_mass = sub["robot0:base_link"]
     assert robot_mass == pytest.approx(70.1294 + 10.7796 + 2.2556 + 0.9087 + 2.5587 + 2.6615 + 2.3311 + 2.1299 + 1.6563 + 1.725 + 0.1354 + 1.5175 +
                                        4 + 4 + 0.002 + 0.0083 + 13.2775, abs=1e-9)
@@ -133,13 +131,10 @@ def test_fetch_closed_form_totals():
     assert hs.fsmooth[d] == pytest.approx(passive_and_act - load, rel=5e-6)
 
 
-@pytest.mark.needs_reference
 def test_invweight0_recomputed_along_a_second_path():
     """dof_invweight0 = diag(M^-1) and the weld's body_invweight0 = block averages of J M^-1 J^T at qpos0 -- recomputed from the C
     oracle's mass matrix and finite-difference Jacobians of its kinematics (the compiler uses analytic Jacobians on the unfused
     tree in numpy), plus the free box whose values are closed-form (1/m and the mean of 1/I)."""
-    import xml.etree.ElementTree as ET
-
     from oracle.oracle_sim import OracleSim
 
     m = load_model("fetch_pick_and_place")
@@ -150,8 +145,7 @@ def test_invweight0_recomputed_along_a_second_path():
     assert np.allclose(np.diag(Minv), m.dof_invweight0, rtol=1e-9)
     # weld robot0:mocap <-> robot0:gripper_link: invweight = that of the gripper link (the mocap body has no dofs)
     site = m.frame_site("robot0:gripper_link")
-    g = next(b for b in ET.parse(os.path.join(REFERENCE_ASSETS, "fetch", "robot.xml")).getroot().iter("body") if b.get("name") == "robot0:gripper_link")
-    ipos = np.array([float(x) for x in g.find("inertial").get("pos").split()])
+    ipos = np.array(FETCH["gripper_link_inertial_pos"])
 
     def com():
         return s.site_xpos[site] + s.site_xmat[site].reshape(3, 3) @ ipos
