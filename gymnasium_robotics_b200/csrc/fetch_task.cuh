@@ -177,6 +177,10 @@ HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, flo
     }
     SYNC();
     LANES(b1, h->nmjb - 1) {
+      if (!stepped) {   // a refresh computes no kinematics: xpos / xquat below would be whatever the shared memory last held
+        for (int k = 0; k < 6; k++) cf[6 * b1 + k] = 0.f;
+        continue;
+      }
       const int b = b1 + 1;      // MJCF body: the row layout of data.cfrc_ext (fused bodies keep their own rows)
       float acc[6] = {0, 0, 0, 0, 0, 0};
       for (int g = 0; g < ngrp; g++) {

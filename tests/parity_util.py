@@ -30,14 +30,17 @@ def oracle_state_record(env, orc):
     return rec
 
 
-def inject_oracle_state(env, oracles):
-    recs = torch.as_tensor(np.stack([oracle_state_record(env, o) for o in oracles]), dtype=torch.float32)
-    env.backend.state.copy_(recs)
-    obs = env.set_state(env.backend.state.clone())
+def inject_oracle_state(env, oracles, rows=None):
+    """Oracle i's state into env row rows[i] (default: row i for every env of the batch); the other rows keep their records."""
+    recs = torch.as_tensor(np.stack([oracle_state_record(env, o) for o in oracles]), dtype=torch.float32).to(env.backend.state.device)
+    rows = slice(None) if rows is None else torch.as_tensor(rows, device=env.backend.state.device)
+    st = env.backend.state.clone()
+    st[rows] = recs
+    obs = env.set_state(st)
     # set_state refreshes derived data, which re-anchors the stored "pose of the welded body as of the last forward
     # pass" to the injected qpos; the oracle's value is one sub-step stale (SURVEY.md Appendix C.1/C.3): restore it
     lay = env.backend.layout
-    env.backend.state[:, lay["pose"]:lay["pose"] + 7] = recs[:, lay["pose"]:lay["pose"] + 7].to(env.backend.state.device)
+    env.backend.state[rows, lay["pose"]:lay["pose"] + 7] = recs[:, lay["pose"]:lay["pose"] + 7]
     return obs
 
 
@@ -62,9 +65,10 @@ def check_envelope(name, errs, p50, p99, mx):
     assert st["p50"] <= p50 and st["p99"] <= p99 and st["max"] <= mx, f"{name}: {st} outside its envelope"
 
 
-def inject_records(env, oracles, extra=None):
+def inject_records(env, oracles, extra=None, rows=None):
     """State records (qpos | qvel | warm start | ctrl [| goal] [| per-env body pose]) from oracle envs that expose `.sim` (families
-    without a mocap weld: Shadow Hand, Adroit, mazes).  `extra(i, oracle, rec, lay)` fills family-specific slots."""
+    without a mocap weld: Shadow Hand, Adroit, mazes).  `extra(i, oracle, rec, lay)` fills family-specific slots.  Without `rows`
+    the result holds one record per oracle; with `rows` it is the env's whole state with oracle i's record in row rows[i]."""
     lay, m = env.backend.layout, env.model
     rec = np.zeros((len(oracles), lay["stride"]))
     for i, o in enumerate(oracles):
@@ -75,4 +79,9 @@ def inject_records(env, oracles, extra=None):
         rec[i, lay["ctrl"]:lay["ctrl"] + m.nu] = s.ctrl
         if extra is not None:
             extra(i, o, rec[i], lay)
-    return torch.as_tensor(rec, dtype=torch.float32, device=env.backend.state.device)
+    recs = torch.as_tensor(rec, dtype=torch.float32, device=env.backend.state.device)
+    if rows is None:
+        return recs
+    st = env.backend.state.clone()
+    st[torch.as_tensor(rows, device=st.device)] = recs
+    return st
