@@ -13,8 +13,9 @@
 #include "step_kernel.cuh"
 #include "reset_sample.cuh"
 
-// warps (= envs) per block: at most 28 (the shared memory of one block); b200sim_create picks the size from the SM count
-#define B200_WPB_MAX 28
+// warps (= envs) per block: at most 32 (the shared memory of one block, for the arm and legged models); b200sim_create picks
+// the size from the SM count
+#define B200_WPB_MAX 32
 
 #ifdef B200_STAGE_TIMING
 extern "C" int b200sim_debug_stage_cycles(unsigned long long* out, int reset) {
@@ -115,7 +116,8 @@ __global__ void reach_reset_kernel(b200sim_reach_reset_t p, unsigned long long s
 
 // ---------------------------------------------------------------------------------------------------------------
 #define B200_FOR_ALL_VARIANTS(X) X(7, 14) X(7, 15) X(7, 21) X(14, 14) X(14, 15) X(14, 21) X(28, 14) X(28, 15) X(28, 21) \
-  X(7, 22) X(14, 22) X(28, 22) X(7, 30) X(14, 30) X(8, 14) X(8, 15) X(8, 21) X(8, 22) X(16, 14) X(16, 15) X(16, 21) X(16, 22)
+  X(7, 22) X(14, 22) X(28, 22) X(7, 30) X(14, 30) X(8, 14) X(8, 15) X(8, 21) X(8, 22) X(16, 14) X(16, 15) X(16, 21) X(16, 22) \
+  X(32, 14) X(32, 15) X(32, 21) X(32, 22)
 
 // wide build (models with 33..40 dofs), compiled from b200sim_wide.cu with 64-bit dof masks
 extern "C" int b200sim_wide_setattr(int wpb, int smem_bytes);
@@ -315,7 +317,7 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
     }
   } else {
     // one block per SM (shared instruction cache), as few waves as the largest fitting block needs, and the smallest block that
-    // needs no more (fewer warps per SM finish sooner): 4096 envs on 132 SMs -> two waves of 16 warps, 1024 envs -> one wave of 8
+    // needs no more (fewer warps per SM finish sooner): 4096 Fetch envs on 132 SMs -> one wave of 32 warps, 1024 envs -> one wave of 8
     auto waves = [&](int w) { return ((num_envs + w - 1) / w + nsm - 1) / nsm; };
     int wmax = 0;
     for (int w = 1; w <= B200_WPB_MAX; w++)

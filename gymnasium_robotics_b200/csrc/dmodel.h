@@ -117,13 +117,14 @@ enum { CX_POS = 0, CX_PAIR = 3, CX_WORDS = 4 };
 enum { DR_DOF = 0, DR_COEF = 1, DR_D = 2, DR_JAR = 3, DR_JV = 4, DR_DOF2 = 5, DR_COEF2 = 6, DR_WORDS = 7 };
 // weld: 6 rows w[6]; D[6], JAR[6] (K*imp*r during set-up), JV[6], B (one value), group
 enum { W_W = 0, W_D = 36, W_JAR = 42, W_JV = 48, W_B = 54, W_GRP = 55, WELD_WORDS = 56 };
-// group = one geom pair in contact (its contacts are contiguous) or one weld: 6x6 block K, contact range, dof mask
-// S = anc(A) xor anc(B) with sign mask (bit set: dof on the B side), a 6-vector used for dV (J*v) and F (J^T f), and the two
-// body ids (A | B << 8; A = body of the pair's first geom) for per-body contact forces (Ant-v5 cfrc_ext)
+// group = one geom pair in contact (its contacts are contiguous) or one weld: one word G_RANGE = first contact | contact count << 8
+// | the two MJCF body ids << 16 (A | B << 8, A = body of the pair's first geom: per-body contact forces, Ant-v5 cfrc_ext), dof
+// mask S = anc(A) xor anc(B) with sign mask (bit set: dof on the B side), a 6-vector used for dV (J*v) and F (J^T f).  The
+// group's 6x6 block K of H is not stored: build_H assembles the blocks in dead solver scratch, as many groups at a time as fit.
 #ifdef B200_WIDE
-enum { G_K = 0, G_START = 21, G_COUNT = 22, G_MASK = 23, G_SIGN = 25, G_V = 27, G_BODIES = 33, GRP_WORDS = 34 };   // two-word masks
+enum { G_RANGE = 0, G_MASK = 1, G_SIGN = 3, G_V = 5, GRP_WORDS = 11 };   // two-word masks
 #else
-enum { G_K = 0, G_START = 21, G_COUNT = 22, G_MASK = 23, G_SIGN = 24, G_V = 25, G_BODIES = 31, GRP_WORDS = 32 };
+enum { G_RANGE = 0, G_MASK = 1, G_SIGN = 2, G_V = 3, GRP_WORDS = 9 };
 #endif
 enum { ROWT_EQ = 0, ROWT_FRICTION = 1, ROWT_LIMIT = 2 };
 enum { CNT_NCON = 0, CNT_NDR = 1, CNT_NGRP = 2, CNT_NCAND = 3, CNT_NWELD = 4, CNT_ITERS = 5, CNT_OVERFLOW = 6 };
@@ -275,7 +276,7 @@ static inline int dm_build(const b200_model_view& m, const double* eq_data_overr
     for (int j = 0; j < m.njnt; j++) if (m.jnt_limited[j] && m.jnt_type[j] != B200_JNT_FREE) nlim++;
     int want = nlim + h.nten;   // at most one side of every limit can be active at a time
     // models with tendon-coupled, friction-loaded joints (the Shadow hand) sit at many limits at once; the arm / legged
-    // models keep the small table that lets 28 envs share one thread block
+    // models keep the small table that lets 32 envs share one thread block
 #ifdef B200_KITCHEN
     for (int e = 0; e < m.neq; e++) if (m.eq_type[e] == B200_EQ_JOINT) want++;   // one (always active) row per joint equality
     if (want > DM_NDOFROW_MIN) h.nten = h.nten > 0 ? h.nten : 0;
@@ -298,7 +299,7 @@ static inline int dm_build(const b200_model_view& m, const double* eq_data_overr
   int nb = h.nb, njnt = h.njnt, nq = h.nq, nv = h.nv, nu = h.nu, ngeom = h.ngeom, nsite = h.nsite, nmocap = h.nmocap,
       neq = h.neq, npair = h.npair, ngridw = h.ngridw, ncon_max = h.ncon_max, ngrp_max = h.ngrp_max, ndr_max = h.ndr_max,
       nten = h.nten, nfric = h.nfric, nsensor = h.nsensor, ncx = h.nsensor > 0 ? h.ncon_max : 0, MW = h.mask_words,
-      grp_words = MW == 2 ? 34 : 32, npenv = h.penv_body > 0 ? 8 : 0, nmjb = h.nmjb;
+      grp_words = MW == 2 ? 11 : 9, npenv = h.penv_body > 0 ? 8 : 0, nmjb = h.nmjb;
 #ifdef B200_HULL
   int nhullv = m.n_hull_vert / 3;
   if (m.n_geom_hull != 2 * m.ngeom) { err = "model blob lacks the hull vertex table (compile with mesh_hull)"; return -1; }
@@ -328,6 +329,10 @@ static inline int dm_build(const b200_model_view& m, const double* eq_data_overr
     int d6off = 16 * nb > nM ? 16 * nb : nM;
     // the line-search edge list (x0, v, D per edge slot) overlays H and d6 after the direction solve
     int need = 3 * (h.edges_per_con * ncon_max + 6 * DM_NWELD_MAX + ndr_max) - 6 * nv;
+    if (need > d6off) d6off = need;
+    // and so do two solver temporaries that are dead by the time H is built: the per-group J qacc of rows_begin (6 per group,
+    // from H's start) and the packed 6x6 blocks of the groups build_H is adding (21 words each after H: room for one at least)
+    need = (nM + 21 > 6 * ngrp_max ? nM + 21 : 6 * ngrp_max) - 6 * nv;
     if (need > d6off) d6off = need;
     d6off = (d6off + 1) & ~1;
     h.s_kinA = u; h.s_kinB = u + 8 * nb;

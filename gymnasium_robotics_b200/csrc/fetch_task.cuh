@@ -163,9 +163,8 @@ HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, flo
     LANES(idx, ngrp * 6) {
       int g = idx / 6, a = idx - 6 * g;
       float* gr = SF(group) + g * GRP_WORDS;
-      const int* gi = (const int*)gr;
       float acc = 0;
-      for (int i = gi[G_START]; i < gi[G_START] + gi[G_COUNT]; i++) {
+      for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
         const float* cr = SF(con) + i * CON_WORDS;
         int dim = con_dim(cr);
         const float* F = cr + C_JV;
@@ -185,9 +184,8 @@ HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, flo
       float acc[6] = {0, 0, 0, 0, 0, 0};
       for (int g = 0; g < ngrp; g++) {
         const float* gr = SF(group) + g * GRP_WORDS;
-        const int* gi = (const int*)gr;
-        if (gi[G_COUNT] == 0) continue;   // weld groups carry no contact
-        int ba = gi[G_BODIES] & 0xff, bb = gi[G_BODIES] >> 8;
+        if (grp_count(gr) == 0) continue;   // weld groups carry no contact
+        int ba = grp_bodies(gr) & 0xff, bb = grp_bodies(gr) >> 8;
         float sg = b == bb ? 1.f : (b == ba ? -1.f : 0.f);
         if (sg != 0.f) for (int k = 0; k < 6; k++) acc[k] += sg * gr[G_V + k];
       }

@@ -203,6 +203,10 @@ HD dmask_t grp_sign(const float* gr) { return ((const uint32_t*)gr)[G_SIGN]; }
 HD void grp_set_masks(int* gi, dmask_t mask, dmask_t sign) { ((uint32_t*)gi)[G_MASK] = mask; ((uint32_t*)gi)[G_SIGN] = sign; }
 #endif
 #define DBIT(m, j) ((int)(((m) >> (j)) & 1))
+// G_RANGE of a group record: first contact (8 bits), contact count (8 bits), MJCF bodies A | B << 8 (16 bits)
+HD int grp_start(const float* gr) { return ((const int*)gr)[G_RANGE] & 0xff; }
+HD int grp_count(const float* gr) { return (((const int*)gr)[G_RANGE] >> 8) & 0xff; }
+HD int grp_bodies(const float* gr) { return (int)(((const uint32_t*)gr)[G_RANGE] >> 16); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // small math
@@ -1386,9 +1390,9 @@ STAGE void collision(const Ctx c) {
       int* gi = (int*)(SF(group) + gid * GRP_WORDS);
       int ba = MI(geom_body)[PAIR_I(pair_geom1)[p]], bb = PAIR_I(pair_geom2)[p] < 0 ? 0 : MI(geom_body)[PAIR_I(pair_geom2)[p]];
       dmask_t ma = DM(body_ancdof, ba), mb = DM(body_ancdof, bb);
-      gi[G_START] = basec + slot; gi[G_COUNT] = kept;
       // the pair's two MJCF (unfused) bodies, A | B << 8 (world / maze walls: 0): rows of per-body contact forces
-      gi[G_BODIES] = GI(geom_mjb)[PAIR_I(pair_geom1)[p]] | ((PAIR_I(pair_geom2)[p] < 0 ? 0 : GI(geom_mjb)[PAIR_I(pair_geom2)[p]]) << 8);
+      const int bodies = GI(geom_mjb)[PAIR_I(pair_geom1)[p]] | ((PAIR_I(pair_geom2)[p] < 0 ? 0 : GI(geom_mjb)[PAIR_I(pair_geom2)[p]]) << 8);
+      ((uint32_t*)gi)[G_RANGE] = (uint32_t)(basec + slot) | (uint32_t)kept << 8 | (uint32_t)bodies << 16;
       grp_set_masks(gi, ma ^ mb, mb);
     }
     if (c.lane == 0) {
@@ -1519,7 +1523,7 @@ STAGE void make_constraint(const Ctx c) {
       ((int*)wr)[W_GRP] = gid;  // one group per weld; row value = w . (V[b1] - V[b2]) => A = b2, B = b1
       int* gi = (int*)(SF(group) + gid * GRP_WORDS);
       dmask_t ma = DM(body_ancdof, b2), mb = DM(body_ancdof, b1);
-      gi[G_START] = 0; gi[G_COUNT] = 0; gi[G_BODIES] = 0;
+      gi[G_RANGE] = 0;
       grp_set_masks(gi, ma ^ mb, mb);
     }
     SYNC();
@@ -1676,14 +1680,15 @@ STAGE void rows_from_vec(const Ctx c, const float* vec) {
 }
 
 // the two row passes that open the solver, fused: rows <- rows + B * (J qvel) + J qacc (same arithmetic and order as
-// two separate passes row += B * (J qvel), row += J qacc); the second group velocity is parked in the group's
-// K block, which build_H fills later)
+// two separate passes row += B * (J qvel), row += J qacc); the second group velocity is parked at 6 g in the H region,
+// which build_H fills later)
 template <bool HF>
 STAGE void rows_begin(const Ctx c, const float* qvel, const float* qacc) {
   ASSUME_SHARED(c);
   ASSUME_SHARED_PTR(qvel); ASSUME_SHARED_PTR(qacc);
   const int* cnt = SI(counters);
   int ngrp = cnt[CNT_NGRP];
+  float* dA = SF(H);
   LANES(idx, ngrp * 6) {
     int g = idx / 6, a = idx - 6 * g;
     float* gr = SF(group) + g * GRP_WORDS;
@@ -1695,30 +1700,32 @@ STAGE void rows_begin(const Ctx c, const float* qvel, const float* qacc) {
       bool pos = DBIT(sg, j);
       acc += pos ? t : -t; acc2 += pos ? t2 : -t2;
     }
-    gr[G_V + a] = acc; gr[G_K + a] = acc2;
+    gr[G_V + a] = acc; dA[idx] = acc2;
   }
   SYNC();
   LANES(i, cnt[CNT_NCON]) {
     float* cr = SF(con) + i * CON_WORDS;
     int dim = con_dim(cr), nbase = dim == 1 ? 1 : dim;
     const float* gr = SF(group) + con_grp(cr) * GRP_WORDS;
+    const float* gA = dA + 6 * con_grp(cr);
     float Bc = cr[C_JV];
     for (int k = 0; k < nbase; k++) {
       float w[6];
       con_w(cr, k, w);
       float u = cr[C_U + k];
       u += Bc * dot6(w, gr + G_V);
-      u += dot6(w, gr + G_K);
+      u += dot6(w, gA);
       cr[C_U + k] = u;
     }
   }
   LANES(i, cnt[CNT_NWELD] * 6) {
     float* wr = SF(weld) + (i / 6) * WELD_WORDS;
     int k = i % 6;
-    const float* gr = SF(group) + ((const int*)wr)[W_GRP] * GRP_WORDS;
+    const int g = ((const int*)wr)[W_GRP];
+    const float* gr = SF(group) + g * GRP_WORDS;
     float u = wr[W_JAR + k];
     u += wr[W_B] * dot6(wr + W_W + 6 * k, gr + G_V);
-    u += dot6(wr + W_W + 6 * k, gr + G_K);
+    u += dot6(wr + W_W + 6 * k, dA + 6 * g);
     wr[W_JAR + k] = u;
   }
   LANES(i, cnt[CNT_NDR]) {
@@ -1782,9 +1789,8 @@ STAGE void pass_F(const Ctx c, float* out) {
   LANES(idx, ngrp * 6) {
     int g = idx / 6, a = idx - 6 * g;
     float* gr = SF(group) + g * GRP_WORDS;
-    const int* gi = (const int*)gr;
     float acc = 0;
-    for (int i = gi[G_START]; i < gi[G_START] + gi[G_COUNT]; i++) {
+    for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
       const float* cr = SF(con) + i * CON_WORDS;
       int dim = con_dim(cr);
       const float* F = cr + C_JV;
@@ -1858,73 +1864,81 @@ STAGE void build_H(const Ctx c) {
   int nv = h->nv, nM = nv * (nv + 1) / 2, nweld = cnt[CNT_NWELD], ngrp = cnt[CNT_NGRP], ndr = cnt[CNT_NDR];
   float* H = SF(H);
   LANES(i, nM) H[i] = SF(M)[i];
-  // K blocks: lane e < 21 owns packed entry e = (r, s) of every group's 6x6
-  LANES(e, 21) {
-    int r = 0; while ((r + 1) * (r + 2) / 2 <= e) r++;
-    const int s = e - r * (r + 1) / 2;
-    for (int g = 0; g < ngrp; g++) {
-      float* K = SF(group) + g * GRP_WORDS + G_K;
-      const int* gi = (const int*)(SF(group) + g * GRP_WORDS);
-      float acc = 0;
-      for (int i = gi[G_START]; i < gi[G_START] + gi[G_COUNT]; i++) {
-        const float* cr = SF(con) + i * CON_WORDS;
-        int dim = con_dim(cr);
-        float D = cr[C_D], un = cr[C_U];
-        float wnr = cr[C_W + r], wns = cr[C_W + s];
-        if (dim == 1) { if (un < 0) acc += D * wnr * wns; continue; }
-        float Wnn = 0;
-        for (int k = 1; k < dim; k++) {
-          float mu = con_mu(cr, k), uk = cr[C_U + k];
-          float ap = (un + mu * uk) < 0 ? 1.f : 0.f, am = (un - mu * uk) < 0 ? 1.f : 0.f;
-          if (ap + am == 0.f) continue;
-          float wkr, wks;
-          if (k < 3) { wkr = cr[C_W + 6 * k + r]; wks = cr[C_W + 6 * k + s]; }
+  // K blocks in the dead solver scratch after H (room for >= 1, dmodel.h), in chunks of as many groups as fit it: every H entry
+  // still sums its groups in ascending order
+  float* Kc = H + nM;
+  const int kcap = (h->s_grad - h->s_H - nM) / 21;
+  for (int g0 = 0; g0 < ngrp; g0 += kcap) {
+    const int g1 = ngrp - g0 < kcap ? ngrp : g0 + kcap;
+    // lane e < 21 owns packed entry e = (r, s) of every group's 6x6
+    LANES(e, 21) {
+      int r = 0; while ((r + 1) * (r + 2) / 2 <= e) r++;
+      const int s = e - r * (r + 1) / 2;
+      for (int g = g0; g < g1; g++) {
+        float* K = Kc + 21 * (g - g0);
+        const float* gr = SF(group) + g * GRP_WORDS;
+        float acc = 0;
+        for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
+          const float* cr = SF(con) + i * CON_WORDS;
+          int dim = con_dim(cr);
+          float D = cr[C_D], un = cr[C_U];
+          float wnr = cr[C_W + r], wns = cr[C_W + s];
+          if (dim == 1) { if (un < 0) acc += D * wnr * wns; continue; }
+          float Wnn = 0;
+          for (int k = 1; k < dim; k++) {
+            float mu = con_mu(cr, k), uk = cr[C_U + k];
+            float ap = (un + mu * uk) < 0 ? 1.f : 0.f, am = (un - mu * uk) < 0 ? 1.f : 0.f;
+            if (ap + am == 0.f) continue;
+            float wkr, wks;
+            if (k < 3) { wkr = cr[C_W + 6 * k + r]; wks = cr[C_W + 6 * k + s]; }
 #ifdef B200_KITCHEN
-          else { wkr = r < 3 ? cr[C_W + 6 * (k - 3) + 3 + r] : 0.f; wks = s < 3 ? cr[C_W + 6 * (k - 3) + 3 + s] : 0.f; }
+            else { wkr = r < 3 ? cr[C_W + 6 * (k - 3) + 3 + r] : 0.f; wks = s < 3 ? cr[C_W + 6 * (k - 3) + 3 + s] : 0.f; }
 #else
-          else { wkr = r < 3 ? cr[C_W + 3 + r] : 0.f; wks = s < 3 ? cr[C_W + 3 + s] : 0.f; }
+            else { wkr = r < 3 ? cr[C_W + 3 + r] : 0.f; wks = s < 3 ? cr[C_W + 3 + s] : 0.f; }
 #endif
-          Wnn += ap + am;
-          float Wnk = mu * (ap - am), Wkk = mu * mu * (ap + am);
-          acc += D * (Wnk * (wnr * wks + wkr * wns) + Wkk * wkr * wks);
+            Wnn += ap + am;
+            float Wnk = mu * (ap - am), Wkk = mu * mu * (ap + am);
+            acc += D * (Wnk * (wnr * wks + wkr * wns) + Wkk * wkr * wks);
+          }
+          acc += D * Wnn * wnr * wns;
         }
-        acc += D * Wnn * wnr * wns;
-      }
-      for (int i = 0; i < nweld; i++) {
-        const float* wr = SF(weld) + i * WELD_WORDS;
-        if (((const int*)wr)[W_GRP] != g) continue;
-        for (int k = 0; k < 6; k++) acc += wr[W_D + k] * wr[W_W + 6 * k + r] * wr[W_W + 6 * k + s];
-      }
-      K[e] = acc;
-    }
-  }
-  SYNC();
-  // lane i owns row i of H: for every group whose chains contain dof i, y = K cdof_i (registers), then
-  // H_ij += sigma_i sigma_j cdof_j . y for the group's dofs j <= i
-  LANES(i, nv) {
-    const float* cd = SF(cdof) + 6 * i;
-    const int row = i * (i + 1) / 2;
-    for (int g = 0; g < ngrp; g++) {
-      const float* gr = SF(group) + g * GRP_WORDS;
-      const dmask_t S = grp_mask(gr), mb = grp_sign(gr);
-      if (!DBIT(S, i)) continue;
-      const float* K = gr + G_K;
-      float y[6];
-#pragma unroll
-      for (int r = 0; r < 6; r++) {
-        float a = 0;
-#pragma unroll
-        for (int s2 = 0; s2 < 6; s2++) a += K[pidx(r, s2)] * cd[s2];
-        y[r] = a;
-      }
-      float si = DBIT(mb, i) ? 1.f : -1.f;
-      dmask_t m2 = S & (((dmask_t)2 << i) - (dmask_t)1);  // j <= i
-      while (m2) {
-        int j = ffs_pop(m2);
-        float sj = DBIT(mb, j) ? 1.f : -1.f;
-        H[row + j] += si * sj * dot6(SF(cdof) + 6 * j, y);
+        for (int i = 0; i < nweld; i++) {
+          const float* wr = SF(weld) + i * WELD_WORDS;
+          if (((const int*)wr)[W_GRP] != g) continue;
+          for (int k = 0; k < 6; k++) acc += wr[W_D + k] * wr[W_W + 6 * k + r] * wr[W_W + 6 * k + s];
+        }
+        K[e] = acc;
       }
     }
+    SYNC();
+    // lane i owns row i of H: for every group whose chains contain dof i, y = K cdof_i (registers), then
+    // H_ij += sigma_i sigma_j cdof_j . y for the group's dofs j <= i
+    LANES(i, nv) {
+      const float* cd = SF(cdof) + 6 * i;
+      const int row = i * (i + 1) / 2;
+      for (int g = g0; g < g1; g++) {
+        const float* gr = SF(group) + g * GRP_WORDS;
+        const dmask_t S = grp_mask(gr), mb = grp_sign(gr);
+        if (!DBIT(S, i)) continue;
+        const float* K = Kc + 21 * (g - g0);
+        float y[6];
+#pragma unroll
+        for (int r = 0; r < 6; r++) {
+          float a = 0;
+#pragma unroll
+          for (int s2 = 0; s2 < 6; s2++) a += K[pidx(r, s2)] * cd[s2];
+          y[r] = a;
+        }
+        float si = DBIT(mb, i) ? 1.f : -1.f;
+        dmask_t m2 = S & (((dmask_t)2 << i) - (dmask_t)1);  // j <= i
+        while (m2) {
+          int j = ffs_pop(m2);
+          float sj = DBIT(mb, j) ? 1.f : -1.f;
+          H[row + j] += si * sj * dot6(SF(cdof) + 6 * j, y);
+        }
+      }
+    }
+    SYNC();
   }
   SYNC();
   // dof friction rows in their quadratic zone (|x| < R * frictionloss)
