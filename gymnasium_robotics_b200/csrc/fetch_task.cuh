@@ -554,7 +554,8 @@ HD void kitchen_observe(const Ctx& c, const FetchTask& t, float* obs, float* ach
 
 // one env, one warp.  `st` is this env's state record; outputs are this env's rows.  `active` is warp-uniform: idle
 // warps run the same control flow (for the block-wide alignment barriers) but touch no memory.
-template <int NVP>
+// REBUILD: rebuild the context before each stage call (stage_ctx)
+template <int NVP, bool REBUILD = false>
 HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, int nraw, float* st, const float* action, float* obs,
                        float* achieved, float* desired, float* reward, float* success, int* iters_out) {
   const DMHead* h = c.h;
@@ -596,18 +597,18 @@ HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, 
   int nsub = mode == MODE_STEP ? t.n_substeps : (mode == MODE_RAW ? nraw : 0);
   for (int s = 0; s < nsub; s++) {
     bool solved = false;
-    forward<NVP>(c, active, h->integrator == B200_INT_RK4 ? nullptr : &solved);
+    forward<NVP, REBUILD>(c, active, h->integrator == B200_INT_RK4 ? nullptr : &solved);
     TIC();
     ALIGN_AT(4); TOC(TM_BARRIER);
-    if (h->integrator == B200_INT_RK4) rk4_substep<NVP>(c, active);
-    else if (active) euler_step<NVP>(c, solved);
+    if (h->integrator == B200_INT_RK4) rk4_substep<NVP, REBUILD>(c, active);
+    else if (active) euler_step<NVP>(stage_ctx<REBUILD>(c), solved);
     TOC(TM_INTEG);
   }
   // touch sensors read the contacts and forces of the last forward pass: a refresh (no sub-step) runs one first,
   // block-uniformly (forward() contains the block-wide alignment barriers); the warm start is left untouched
   const bool touch_fwd = NVP >= 30 && ((t.kind == TASK_HAND && t.touch_mode != 0) || t.kind == TASK_ADROIT_HAMMER) && nsub == 0;
   if (touch_fwd) {
-    forward<NVP>(c, active);
+    forward<NVP, REBUILD>(c, active);
     if (active) { LANES(i, h->nv) SF(qacc)[i] = st[t.st_warm + i]; SYNC(); }
   }
   if (!active) return;

@@ -119,6 +119,32 @@ enum { TM_KIN = 0, TM_COM_M, TM_COLL, TM_CONSTR, TM_SMOOTH, TM_NBEGIN, TM_NCHECK
 #define TIC() do { } while (0)
 #define TOC(k) do { } while (0)
 #endif
+#ifdef __CUDACC__
+// the step kernel's dynamic shared memory (`smem` in step_kernel.cuh): model header + HOT arrays, then one scratch per warp
+extern __shared__ __align__(128) uint32_t b200_smem[];
+#endif
+// The context handed to a stage call by the driver loops (forward(), the sub-step loop of fetch_env_step).  In a block of 28 or
+// 32 warps a thread gets at most 72 / 64 registers, and the stages use nearly all of them, so a scratch pointer the driver kept
+// live across the ~50 stage calls of a sub-step was spilled to local memory (which, beside a 231 KB shared-memory carve-out, is
+// L2) and reloaded after every call.  There (REBUILD) the driver rebuilds the context before each call instead, from the header
+// words in shared memory and the warp index.  With 128 registers nothing is spilled and the rebuild only adds instructions
+// (FetchPickAndPlace at 32 warps: -6 % step-kernel time; the 7..16-warp kernels were slower with it, DESIGN.md section 6).
+template <bool REBUILD>
+HD Ctx stage_ctx(const Ctx& c) {
+#ifdef __CUDACC__
+  if (REBUILD) {
+    // (%tid.x read afresh: threadIdx.x would be merged with the kernel's own lane and warp values, which then stay live)
+    uint32_t tid;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+    Ctx r = c;
+    const DMHead* h = (const DMHead*)b200_smem;
+    r.s = (float*)(b200_smem + h->hot_words) + (tid >> 5) * h->scr_words;
+    r.lane = (int)(tid & 31);
+    return r;
+  }
+#endif
+  return c;
+}
 #define MI(name) ((const int*)(c.mw + c.h->o_##name))
 #define MU(name) ((const uint32_t*)(c.mw + c.h->o_##name))
 #define MF(name) ((const float*)(c.mw + c.h->o_##name))
@@ -2382,7 +2408,7 @@ STAGE void euler_solve(const Ctx c) {
 // Newton solve has converged then runs the (M + h B) solve of that step while the other warps of the block run their next
 // Newton direction solve -- the same routine (spd_solve<NVP>), i.e. the same code window -- instead of idling at the barrier;
 // *euler_solved tells euler_step that SF(search) already holds the solution.
-template <int NVP>
+template <int NVP, bool REBUILD = false>
 HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
   constexpr bool HF = NVP >= 30;
   constexpr bool CX = NVP == 22 || NVP >= 30;   // NVP 22 = the 21-dof arm build plus the convex collider (FetchSlide)
@@ -2391,38 +2417,38 @@ HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
 #ifndef B200_NO_ALIGN_FIRST
   ALIGN_AT(1); TOC(TM_BARRIER);
 #endif
-  if (active) kinematics(c);
+  if (active) kinematics(stage_ctx<REBUILD>(c));
   TOC(TM_KIN); ALIGN_AT(4); TOC(TM_BARRIER);
-  if (active) { com_quantities(c); mass_matrix(c); }
+  if (active) { com_quantities(stage_ctx<REBUILD>(c)); mass_matrix(stage_ctx<REBUILD>(c)); }
 #ifndef B200_NO_ALIGN_PRECOLL
   TOC(TM_COM_M); ALIGN_AT(2); TOC(TM_BARRIER);
 #endif
-  if (active) collision<HF, CX>(c);
+  if (active) collision<HF, CX>(stage_ctx<REBUILD>(c));
   TOC(TM_COLL); ALIGN_AT(2); TOC(TM_BARRIER);
-  if (active) make_constraint<HF>(c);
+  if (active) make_constraint<HF>(stage_ctx<REBUILD>(c));
   TOC(TM_CONSTR); ALIGN_AT(4); TOC(TM_BARRIER);
-  if (active) smooth_forces(c);
+  if (active) smooth_forces(stage_ctx<REBUILD>(c));
   TOC(TM_SMOOTH); ALIGN_AT(4); TOC(TM_BARRIER);
-  if (active) newton_begin<HF>(c);
+  if (active) newton_begin<HF>(stage_ctx<REBUILD>(c));
   TOC(TM_NBEGIN);
   int done = active ? 0 : 1;
   float improvement = 0;
   if (kAlign >= 3) {
     for (int iter = 0;; iter++) {
       ALIGN(); TOC(TM_BARRIER);
-      if (!done) done = newton_check<HF>(c, iter, improvement);
+      if (!done) done = newton_check<HF>(stage_ctx<REBUILD>(c), iter, improvement);
       TOC(TM_NCHECK);
       bool more = ALIGN_OR(!done);
       TOC(TM_BARRIER);
       if (!more) break;
-      if (!done) build_H<HF>(c);
+      if (!done) build_H<HF>(stage_ctx<REBUILD>(c));
       TOC(TM_BUILDH); ALIGN_AT(4); TOC(TM_BARRIER);
-      if (!done) newton_direction<NVP>(c);
+      if (!done) newton_direction<NVP>(stage_ctx<REBUILD>(c));
 #ifdef B200_EULER_PIGGYBACK
-      else if (euler_solved && active && !*euler_solved && c.h->any_damping) { euler_solve<NVP>(c); *euler_solved = true; }
+      else if (euler_solved && active && !*euler_solved && c.h->any_damping) { euler_solve<NVP>(stage_ctx<REBUILD>(c)); *euler_solved = true; }
 #endif
       TOC(TM_NDIR); ALIGN(); TOC(TM_BARRIER);
-      if (!done) done = newton_move<HF>(c, &improvement) ? 2 : 0;
+      if (!done) done = newton_move<HF>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
       TOC(TM_NMOVE);
     }
   } else {
@@ -2483,7 +2509,7 @@ STAGE void euler_step(const Ctx c, bool solved = false) {
 // one classical RK4 sub-step over (qpos, qvel), ctrl held constant, one forward pass per stage, no implicit damping
 // (reference: `integrator="RK4"` of the Ant model, gymnasium_robotics/envs/mujoco/assets/ant.xml:3).  The first
 // stage's forward pass has already been done by the caller.
-template <int NVP>
+template <int NVP, bool REBUILD = false>
 HD void rk4_substep(const Ctx c, bool active) {
   const DMHead* h = c.h;
   const int nv = h->nv, nq = h->nq;
@@ -2503,7 +2529,7 @@ HD void rk4_substep(const Ctx c, bool active) {
       LANES(i, nv) SF(qvel)[i] = SF(rk_v0)[i] + a * SF(qacc)[i];
       SYNC();
     }
-    forward<NVP>(c, active);
+    forward<NVP, REBUILD>(c, active);
     if (active) {
       LANES(i, nv) { SF(rk_dx)[i] += B[st] * SF(qvel)[i]; SF(rk_df)[i] += B[st] * SF(qacc)[i]; }
       SYNC();

@@ -73,7 +73,8 @@ __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restr
   const float* act = io.actions ? io.actions + e * task.nact : nullptr;  // only dereferenced in MODE_STEP by active warps
   float* success = io.success + e * io.scalar_stride;
   int iters = 0;
-  fetch_env_step<NVP>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
+  // (WPB >= 28: at most 72 registers per thread, the driver rebuilds its context before each stage call -- stage_ctx)
+  fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
                       io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters);
   if (active && lane == 0) {
     // episode bookkeeping of the env-step (TimeLimit wrapper + compute_terminated), flags in both output forms; refresh / raw
