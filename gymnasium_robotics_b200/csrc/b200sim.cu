@@ -296,6 +296,13 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   if ((t.kind == TASK_HAND || t.kind == TASK_HAND_REACH || TASK_IS_ADROIT(t.kind)) && h->nvp < 30) h->nvp = 30;  // the hand task code is compiled into this build only
   if (dh->nv <= 21 && dh->any_convex_pair) h->nvp = 22;  // arm build that carries the general convex collider (FetchSlide's puck)
   if (dh->nv <= 21 && (dh->nten > 0 || dh->nfric > 0 || dh->nsensor > 0 || dh->any_round_pair)) h->nvp = 30;  // hand features live in the NVP = 30 build
+  // the line search keeps the env's constraint edges in registers: refuse a model with more edge slots than its kernel build holds
+  // (the kitchen builds check their own capacity in dm_build)
+  if (!h->kitchen && dm_ls_edges(*dh) > 32 * DM_LS_E(h->nvp)) {
+    std::string m = "b200sim_create: the line search of the NVP = " + std::to_string(h->nvp) + " kernel build holds " + std::to_string(32 * DM_LS_E(h->nvp)) +
+                    " constraint edges per env, this model needs up to " + std::to_string(dm_ls_edges(*dh));
+    delete h; return fail(nullptr, m, -8);
+  }
   auto fits = [&](int w) { return ((size_t)dh->hot_words + (size_t)w * dh->scr_words) * 4 + 64 <= 232448; };
   auto built = [&](int w) {   // an instantiation <w, nvp> exists (the wide ones: b200sim_wide.cu)
     if (h->nvp == B200_WIDE_NVP) return w == 7 || w == 10 || w == 13 || w == 14;

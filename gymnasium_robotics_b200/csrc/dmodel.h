@@ -23,6 +23,15 @@
 // words).  The slots overlay scratch that is dead while the narrow phase runs: region A = the body-force / dof-term buffers of the
 // smooth-force stage (b6 .. d6), region B = the contact records, as long as the narrow phase has not written one.
 #define DM_CSLOT_WORDS 40
+// Line-search edge slots per lane of a 32-lane warp, per kernel build: sim_core.cuh `linesearch` keeps every constraint edge of
+// the env in registers, edge e in slot e / 32 of lane e % 32.  The arm and legged builds (NVP <= 22) carry at most 20 contacts
+// of 6 pyramid edges, one weld (6 rows) and 8 dof rows = 134 edges; the hand and Adroit builds (NVP 30, 36; 32 in the test
+// emulation) up to 48 dof rows = 174.  dm_ls_edges() is a model's bound.  The kitchen builds keep a shared-memory edge list.
+#ifdef B200_KITCHEN
+#define DM_LS_E(NVP) 0
+#else
+#define DM_LS_E(NVP) ((NVP) >= 30 ? 6 : 5)
+#endif
 
 // (name, words-per-element, kind) ; kind selects the element count.  HOT arrays are staged into shared memory by every
 // block; COLD arrays (per-pair contact parameters, read only when a contact is created) stay in global memory.
@@ -159,6 +168,8 @@ struct DMHead {
 // ---------------------------------------------------------------------------------------------------------------
 // host-side builder
 static inline uint32_t f2w(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+// most line-search edges an env of this model can have: every contact with the widest pyramid, the welds, the dof rows
+static inline int dm_ls_edges(const DMHead& h) { return h.edges_per_con * h.ncon_max + 6 * DM_NWELD_MAX + h.ndr_max; }
 
 static inline int dm_build(const b200_model_view& m, const double* eq_data_override, const float ref[3],
                            std::vector<uint32_t>& buf, std::string& err, int penv_body = -1, bool force_wide = false,
@@ -327,7 +338,9 @@ static inline int dm_build(const b200_model_view& m, const double* eq_data_overr
     so = (so + 3) & ~3;   // 16-byte aligned: the register Cholesky reads its column buffers (in the dead H region) as float4
     int nM = nv * (nv + 1) / 2, u = so;
     int d6off = 16 * nb > nM ? 16 * nb : nM;
-    // the line-search edge list (x0, v, D per edge slot) overlays H and d6 after the direction solve
+    // room for a line-search edge list (x0, v, D per edge slot) over H and d6.  Only the kitchen builds still use it (the others keep
+    // their edges in registers); it stays for all because it sizes this region for AntMaze and PointMaze too, and with it their
+    // scratch (scr_words, hence the accepted block sizes) and their narrow-phase slots in region A
     int need = 3 * (h.edges_per_con * ncon_max + 6 * DM_NWELD_MAX + ndr_max) - 6 * nv;
     if (need > d6off) d6off = need;
     // and so do two solver temporaries that are dead by the time H is built: the per-group J qacc of rows_begin (6 per group,
@@ -504,7 +517,10 @@ static inline int dm_build(const b200_model_view& m, const double* eq_data_overr
     F(h.o_bg_radius, g, bgs[g].r);
   }
 #endif
-  if (3 * (h.edges_per_con * ncon_max + 6 * DM_NWELD_MAX + ndr_max) > h.s_grad - h.s_H) { err = "line-search edge list does not fit the solver scratch"; return -1; }
+#ifdef B200_KITCHEN
+  // the kitchen builds' line search walks an edge list in the solver scratch (the other builds are checked by b200sim_create)
+  if (3 * dm_ls_edges(h) > h.s_grad - h.s_H) { err = "line-search edge list does not fit the solver scratch"; return -1; }
+#endif
   for (int k = 0; k < nsensor; k++) {
     I(h.o_sensor_site, k, m.sensor_site[k]); I(h.o_sensor_body, k, m.sensor_body[k]); I(h.o_sensor_type, k, m.sensor_type[k]);
     for (int a = 0; a < 3; a++) F(h.o_sensor_size, 3 * k + a, m.sensor_size[3 * k + a]);

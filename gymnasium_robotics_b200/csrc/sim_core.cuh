@@ -2211,9 +2211,120 @@ static inline void spd_solve(const Ctx& c, const float* A, const float* dadd, fl
 }
 #endif
 
-// Line search over a flat edge list.  ls_edges() expands every constraint row into (x0, v, D) triples once per Newton
-// move -- pyramid edges of a contact are x = u_n +- mu u_k -- into the scratch that H and d6 occupied before the direction
-// solve; ls_eval() then walks the triples with all 32 lanes.  D < 0 marks a two-sided (equality) row, D == 0 an empty slot.
+// the step alpha and the improvement cost(0) - cost(alpha), returned by value (the caller's improvement lives on its stack)
+struct LsStep { float alpha, improve; };
+#ifndef B200_KITCHEN
+// Line search over the constraint edges, held in registers.  Every constraint row expands into one or more edges (x0, v, D):
+// the pyramid edges of a contact are x = u_n +- mu u_k, then come the six rows of each weld and the dof rows.  D < 0 marks a
+// two-sided (equality) row, D == 0 an empty slot (a contact's unused pyramid edges, and the slots past the last edge).  Lane
+// `lane` owns edge slots lane + WARP_W j, j < LSE * 32 / WARP_W -- the lane assignment of a strided loop over the edges -- and
+// builds them once per Newton move; every cost evaluation then reads them from registers.  LSE (edge slots per lane of a
+// 32-lane warp) is fixed per kernel build (dmodel.h DM_LS_E); b200sim_create refuses models with more edges than that.
+struct LsVal { float cost, d1, d2; };
+
+// x_n + mu (+-x_k), rounded once on the device (nvcc has always fused this product into the addition, FFMA) and twice on the host
+// (ISO C++ does not contract): the register build keeps the edge values of both bit for bit, whatever the surrounding code
+HD float pyramid_edge(float xn, float mu, float xk) {
+#ifdef __CUDACC__
+  return fmaf(mu, xk, xn);
+#else
+  return xn + mu * xk;
+#endif
+}
+
+// cost(alpha) - gauss constant, first and second derivative.  Each lane adds its slots in ascending order, as the strided loop
+// over a shared edge list did, so the sums do not depend on where the edges are kept.
+template <bool HF, int NS>
+HD LsVal ls_eval(const Ctx c, const float (&ex)[NS], const float (&ev)[NS], const float (&eD)[NS], int nedge, float alpha, float g1,
+                 float g2) {
+  float cost = 0, d1 = 0, d2 = 0;
+#pragma unroll
+  for (int j = 0; j < NS; j++) {
+    if (WARP_W * j >= nedge) break;   // warp-uniform: no lane has an edge in slot j or later
+    float x0 = ex[j], v = ev[j], D = eD[j];
+    float x = fmaf(alpha, v, x0), Da = fabsf(D);
+    if (D < 0 || (x < 0 && D > 0)) { float dx = Da * x; cost = fmaf(0.5f * dx, x, cost); d1 = fmaf(dx, v, d1); d2 = fmaf(Da * v, v, d2); }
+  }
+  if (HF) LANES(d, c.h->nfric) {
+    float D = MF(dof_fricD)[d];
+    if (D > 0) {
+      float fl = MF(dof_frictionloss)[d], v = SF(fric)[c.h->nfric + d], x = SF(fric)[d] + alpha * v, Rf = fl / D;
+      if (x <= -Rf) { cost += fl * (-0.5f * Rf - x); d1 -= fl * v; }
+      else if (x >= Rf) { cost += fl * (-0.5f * Rf + x); d1 += fl * v; }
+      else { cost += 0.5f * D * x * x; d1 += D * x * v; d2 += D * v * v; }
+    }
+  }
+  LsVal r;
+  r.cost = wsum(cost) + alpha * g1 + alpha * alpha * g2;
+  r.d1 = wsum(d1) + g1 + 2 * alpha * g2;
+  r.d2 = wsum(d2) + 2 * g2;
+  return r;
+}
+
+// inlined into newton_move: one call boundary less per move (the 32-warp kernels run 1 % faster than with a call of its own)
+template <bool HF, int LSE>
+HD LsStep linesearch(const Ctx c, float g1, float g2, float gtol, int maxit) {
+  ASSUME_SHARED(c);
+  constexpr int NS = LSE * 32 / WARP_W;   // slots per lane
+  const DMHead* h = c.h;
+  const int* cnt = SI(counters);
+  const int epc = h->edges_per_con, ncon = cnt[CNT_NCON], nweld6 = cnt[CNT_NWELD] * 6, ndr = cnt[CNT_NDR];
+  const int nce = epc * ncon, nwe = nce + nweld6, nedge = nwe + ndr;
+  float ex[NS], ev[NS], eD[NS];
+  // contact and pyramid edge of slot j, q = e / epc and r = e % epc, advanced by WARP_W per slot (two divisions in all)
+  const int qs = WARP_W / epc, rs = WARP_W % epc;
+  int q = c.lane / epc, r = c.lane % epc;
+#pragma unroll
+  for (int j = 0; j < NS; j++) {
+    const int e = c.lane + WARP_W * j;
+    float x0 = 0.f, v = 0.f, D = 0.f;
+    if (j > 0) { q += qs; r += rs; if (r >= epc) { r -= epc; q++; } }
+    if (WARP_W * j < nedge) {   // warp-uniform: slots past the last edge stay empty
+      if (e < nce) {   // contact q, pyramid edge r = base row 1 + r / 2, + for even r
+        const float* cr = SF(con) + q * CON_WORDS;
+        const int k = r, dim = con_dim(cr);
+        const float un = cr[C_U], vn = cr[C_JV];
+        if (dim == 1) {
+          if (k == 0) { x0 = un; v = vn; D = cr[C_D]; }
+        } else if (k < 2 * (dim - 1)) {
+          const int b = 1 + (k >> 1);
+          const float mu = con_mu(cr, b), su = (k & 1) ? -cr[C_U + b] : cr[C_U + b], sv = (k & 1) ? -cr[C_JV + b] : cr[C_JV + b];
+          x0 = pyramid_edge(un, mu, su); v = pyramid_edge(vn, mu, sv);
+          D = cr[C_D];
+        }
+      } else if (e < nwe) {
+        const int i = e - nce;
+        const float* wr = SF(weld) + (i / 6) * WELD_WORDS;
+        x0 = wr[W_JAR + i % 6]; v = wr[W_JV + i % 6]; D = -wr[W_D + i % 6];
+      } else if (e < nedge) {
+        const float* dr = SF(dofrow) + (e - nwe) * DR_WORDS;
+        x0 = dr[DR_JAR]; v = dr[DR_JV]; D = dr[DR_D];
+      }
+    }
+    ex[j] = x0; ev[j] = v; eD[j] = D;
+  }
+  const LsVal p0 = ls_eval<HF>(c, ex, ev, eD, nedge, 0.f, g1, g2);
+  if (p0.d1 >= 0 || p0.d2 <= 0) return LsStep{0.f, 0.f};
+  gtol = fmaxf(gtol, 1e-5f * fabsf(p0.d1));  // single-precision floor on the derivative test
+  float lo = 0, hi = -1, alpha = -p0.d1 / p0.d2, best = 0, bestcost = p0.cost;
+  for (int it = 0; it < maxit; it++) {
+    const LsVal p = ls_eval<HF>(c, ex, ev, eD, nedge, alpha, g1, g2);
+    if (p.cost <= bestcost) { bestcost = p.cost; best = alpha; }
+    if (fabsf(p.d1) < gtol) break;
+    if (p.d1 < 0) lo = alpha; else hi = alpha;
+    float next = alpha - p.d1 / p.d2;
+    if (hi > 0 && (next <= lo || next >= hi)) next = 0.5f * (lo + hi);
+    if (next == alpha) break;
+    alpha = next;
+  }
+  return LsStep{best, p0.cost - bestcost};
+}
+
+#else
+// The kitchen builds (B200_KITCHEN) keep the line search over a flat edge list in shared memory: with up to 10 edges per contact
+// the register version above ran their step kernel 1.6 % slower (DESIGN.md section 3).  ls_edges() expands every constraint row
+// into (x0, v, D) triples once per Newton move into the scratch that H and d6 occupied before the direction solve; ls_eval()
+// then walks the triples with all 32 lanes.  LSE is unused here.
 template <bool HF>
 STAGE int ls_edges(const Ctx c) {
   ASSUME_SHARED(c);
@@ -2275,15 +2386,13 @@ STAGE void ls_eval(const Ctx c, int nedge, float alpha, float g1, float g2, floa
   out[2] = wsum(d2) + 2 * g2;
 }
 
-// returns alpha; *improve = cost(0) - cost(alpha)
-template <bool HF>
-STAGE float linesearch(const Ctx c, float g1, float g2, float gtol, int maxit, float* improve) {
+template <bool HF, int LSE>
+STAGE LsStep linesearch(const Ctx c, float g1, float g2, float gtol, int maxit) {
   ASSUME_SHARED(c);
   float p0[3], p[3];
   const int nedge = ls_edges<HF>(c);
   ls_eval<HF>(c, nedge, 0.f, g1, g2, p0);
-  *improve = 0;
-  if (p0[1] >= 0 || p0[2] <= 0) return 0.f;
+  if (p0[1] >= 0 || p0[2] <= 0) return LsStep{0.f, 0.f};
   gtol = fmaxf(gtol, 1e-5f * fabsf(p0[1]));  // single-precision floor on the derivative test
   float lo = 0, hi = -1, alpha = -p0[1] / p0[2], best = 0, bestcost = p0[0];
   for (int it = 0; it < maxit; it++) {
@@ -2296,9 +2405,10 @@ STAGE float linesearch(const Ctx c, float g1, float g2, float gtol, int maxit, f
     if (next == alpha) break;
     alpha = next;
   }
-  *improve = p0[0] - bestcost;
-  return best;
+  return LsStep{best, p0[0] - bestcost};
 }
+
+#endif
 
 // Newton solver, split so that the iteration loop can be driven block-uniformly (see forward()).
 template <bool HF>
@@ -2349,7 +2459,7 @@ STAGE void newton_direction(const Ctx c) {
 }
 
 // exact line search and move; returns 1 when the solver must stop (no progress possible), *improvement updated
-template <bool HF>
+template <bool HF, int LSE>
 STAGE int newton_move(const Ctx c, float* improvement) {
   ASSUME_SHARED(c);
   const DMHead* h = c.h;
@@ -2368,7 +2478,9 @@ STAGE int newton_move(const Ctx c, float* improvement) {
   if (sn < 1e-20f) return 1;
   float gtol = h->tolerance * h->ls_tolerance * sn / scale;
   TOC(TM_MV_ROWS);
-  float alpha = linesearch<HF>(c, q1, q2, gtol, h->ls_iterations < 20 ? h->ls_iterations : 20, improvement);
+  const LsStep ls = linesearch<HF, LSE>(c, q1, q2, gtol, h->ls_iterations < 20 ? h->ls_iterations : 20);
+  *improvement = ls.improve;
+  const float alpha = ls.alpha;
   TOC(TM_MV_LS);
   if (alpha == 0.f) return 1;
   LANES(i, nv) { a[i] += alpha * search[i]; Ma[i] += alpha * Mv[i]; }
@@ -2413,6 +2525,7 @@ HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
   constexpr bool HF = NVP >= 30;
   constexpr bool CX = NVP == 22 || NVP >= 30;   // NVP 22 = the 21-dof arm build plus the convex collider (FetchSlide)
   constexpr int kAlign = ALIGN_LEVEL_FOR(NVP);
+  constexpr int kLsE = DM_LS_E(NVP);   // line-search edge slots per lane
   TIC();
 #ifndef B200_NO_ALIGN_FIRST
   ALIGN_AT(1); TOC(TM_BARRIER);
@@ -2448,7 +2561,7 @@ HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
       else if (euler_solved && active && !*euler_solved && c.h->any_damping) { euler_solve<NVP>(stage_ctx<REBUILD>(c)); *euler_solved = true; }
 #endif
       TOC(TM_NDIR); ALIGN(); TOC(TM_BARRIER);
-      if (!done) done = newton_move<HF>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
+      if (!done) done = newton_move<HF, kLsE>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
       TOC(TM_NMOVE);
     }
   } else {
@@ -2458,7 +2571,7 @@ HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
       if (done) break;
       build_H<HF>(c);
       newton_direction<NVP>(c);
-      done = newton_move<HF>(c, &improvement) ? 2 : 0;
+      done = newton_move<HF, kLsE>(c, &improvement) ? 2 : 0;
     }
   }
 }
