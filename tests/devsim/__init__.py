@@ -1,0 +1,74 @@
+"""Test-only ctypes wrapper for the device harness (devsim.cu): single stages of the kernel source on the GPU.
+
+One shared library per product translation unit, built with the product's nvcc flags and that unit's defines, so that each
+stage runs in exactly the instantiation and arithmetic the product kernels use (nvcc's FMA contraction, -prec-div=false,
+-prec-sqrt=false, the hardware rsqrtf).  nvcc cross-compiles them without a GPU; running them needs one.
+"""
+from __future__ import annotations
+
+import ctypes
+import os
+import subprocess
+
+import numpy as np
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_ROOT = os.path.dirname(os.path.dirname(_HERE))
+_LIB = {}
+
+# flavor -> (the product translation unit it mirrors, its extra defines, the NVPs that unit instantiates)
+FLAVORS = {
+    "plain": ("b200sim.cu", [], (14, 15, 21, 22, 30)),
+    "wide": ("b200sim_wide.cu", ["-DB200_WIDE"], (36,)),
+    "kitchen": ("b200sim_kitchen.cu", ["-DB200_KITCHEN"], (31,)),
+}
+NVP_FLAVOR = {v: f for f, (_, _, vs) in FLAVORS.items() for v in vs}
+
+
+def build(flavor="plain", force=False):
+    """Compile libdevsim_<flavor>.so (lazily, under a file lock, into a temporary name renamed into place)."""
+    from gymnasium_robotics_b200 import _lib
+
+    out = os.path.join(_HERE, f"libdevsim_{flavor}.so")
+    csrc = os.path.join(_ROOT, "gymnasium_robotics_b200", "csrc")
+    srcs = [os.path.join(_HERE, "devsim.cu")] + [os.path.join(csrc, f) for f in ("sim_core.cuh", "dmodel.h", "fetch_task.cuh")] + \
+           [os.path.join(_ROOT, "include", f) for f in ("b200sim_model.h", "b200sim.h")]
+
+    def stale():
+        return force or not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(s) for s in srcs)
+
+    if stale():
+        import fcntl
+
+        with open(out + ".lock", "w") as lk:
+            fcntl.flock(lk, fcntl.LOCK_EX)
+            if stale():
+                tmp = f"{out}.{os.getpid()}.tmp"
+                subprocess.check_call(["nvcc"] + list(_lib.NVCC_FLAGS) + FLAVORS[flavor][1] + ["-o", tmp, srcs[0]])
+                os.replace(tmp, out)
+                force = False
+    return out
+
+
+def lib(flavor="plain"):
+    if _LIB.get(flavor) is None:
+        L = ctypes.CDLL(build(flavor))
+        vp, ci = ctypes.c_void_p, ctypes.c_int
+        L.devsim_spd.argtypes = [ci, ci, vp, vp, vp, ctypes.c_float, ci, vp, vp, ci, ci, ci, ci]
+        L.devsim_spd.restype = ci
+        L.devsim_last_error.restype = ctypes.c_char_p
+        _LIB[flavor] = L
+    return _LIB[flavor]
+
+
+def spd(nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
+    """spd_solve<nvp> on the GPU for a batch of cases, one block each.  nv: [n] int; A: [n, la], x and dadd: [n, lx], H: [n, lh]
+    float32 buffers (la, lx, lh multiples of 4).  A, x and H are overwritten with their contents after the solve."""
+    L = lib(NVP_FLAVOR[nvp])
+    nv = np.ascontiguousarray(nv, dtype=np.int32)
+    for a in (A, x, dadd, H):
+        assert a.dtype == np.float32 and a.flags.c_contiguous and a.shape[0] == len(nv) and a.shape[1] % 4 == 0
+    rc = L.devsim_spd(int(nvp), len(nv), nv.ctypes.data, A.ctypes.data, dadd.ctypes.data, float(hh), int(bool(use_dadd)), x.ctypes.data,
+                      H.ctypes.data, A.shape[1], x.shape[1], H.shape[1], int(bool(inplace)))
+    if rc != 0:
+        raise RuntimeError(f"devsim_spd(nvp={nvp}): {L.devsim_last_error().decode()}")

@@ -87,9 +87,22 @@ def lib(wide=False):
         L.hostsim_offset.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
         L.hostsim_scr_words.argtypes = [ctypes.c_void_p]
         L.hostsim_env_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 7
+        L.hostsim_spd.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
+        L.hostsim_spd.restype = ctypes.c_int
         assert L.hostsim_task_size() == ctypes.sizeof(FetchTaskC)
         _LIB[wide] = L
     return _LIB[wide]
+
+
+def spd(flavor, nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
+    """spd_solve<nvp> of the given flavor (on the 32-lane flavors the register Cholesky, bordered for nvp > 32) for a batch of cases,
+    one call each; the same buffers as tests.devsim.spd.  A, x and H are overwritten with their contents after the solve."""
+    L = lib(wide=flavor)
+    for e in range(len(nv)):
+        pa, px, ph = A[e].ctypes.data, x[e].ctypes.data, H[e].ctypes.data
+        rc = L.hostsim_spd(int(nvp), int(nv[e]), pa, dadd[e].ctypes.data if use_dadd else None, float(hh), px, pa if inplace else ph)
+        if rc != 0:
+            raise RuntimeError(f"hostsim_spd: flavor {flavor!r} does not instantiate NVP {nvp}")
 
 
 class HostSim:

@@ -6,6 +6,7 @@
 #include <cstring>
 #include <vector>
 #include <string>
+#include <type_traits>
 #ifdef B200_HOST_WARP
 #include "hostwarp.h"   // WARP_W == 32: the lane-parallel code paths on 32 lock-step fibers
 #endif
@@ -37,6 +38,15 @@ template <class F> static void warp_call(const Ctx& base, F f) {
 static const bool kWide = true;   // 64-bit dof masks: the tables carry two words per mask
 #else
 static const bool kWide = false;
+#endif
+// the padded dof count of the product kernel build this flavor stands for: the wide build's bordered Cholesky (32 + 4 rows), the
+// kitchen builds' 31, else 32 (the WARP_W == 1 flavors solve with the shared-memory Cholesky whatever the size)
+#if defined(B200_WIDE)
+#define HOST_NVP 36
+#elif defined(B200_KITCHEN)
+#define HOST_NVP 31
+#else
+#define HOST_NVP 32
 #endif
 
 struct HostSim {
@@ -76,17 +86,50 @@ int hostsim_offset(void* p, const char* name) {
 #undef X
   return -1;
 }
-void hostsim_forward(void* p) { warp_call(((HostSim*)p)->ctx, [](const Ctx& c) { forward<32>(c, true); }); }
-void hostsim_step(void* p, int n) { warp_call(((HostSim*)p)->ctx, [n](const Ctx& c) { for (int i = 0; i < n; i++) { forward<32>(c, true); euler_step<32>(c); } }); }
+void hostsim_forward(void* p) { warp_call(((HostSim*)p)->ctx, [](const Ctx& c) { forward<HOST_NVP>(c, true); }); }
+void hostsim_step(void* p, int n) { warp_call(((HostSim*)p)->ctx, [n](const Ctx& c) { for (int i = 0; i < n; i++) { forward<HOST_NVP>(c, true); euler_step<HOST_NVP>(c); } }); }
 void hostsim_kinematics(void* p) { warp_call(((HostSim*)p)->ctx, [](const Ctx& c) { kinematics(c); com_quantities(c); mass_matrix(c); }); }
 int hostsim_task_size() { return (int)sizeof(FetchTask); }
 int hostsim_env_step(void* p, const FetchTask* t, int mode, int nraw, float* st, const float* action, float* obs, float* achieved,
                      float* desired, float* reward, float* success) {
   int it = 0;
   warp_call(((HostSim*)p)->ctx, [&](const Ctx& c) {
-    fetch_env_step<32>(c, *t, true, mode, nraw, st, action, obs, achieved, desired, reward, success, &it);
+    fetch_env_step<HOST_NVP>(c, *t, true, mode, nraw, st, action, obs, achieved, desired, reward, success, &it);
   });
   return it;
+}
+// x <- (A + hh diag(dadd))^-1 x with spd_solve<nvp> for an nv-dof system: A packed lower-triangular (nv (nv + 1) / 2 words), dadd
+// optional, scratchH the solver's work area (the column buffers of the register Cholesky); A == scratchH is the Newton solve's
+// in-place call.  Only the header's nv is read.  Returns -1 for an nvp this flavor does not instantiate.
+int hostsim_spd(int nvp, int nv, const float* A, const float* dadd, float hh, float* x, float* scratchH) {
+  DMHead head;
+  memset(&head, 0, sizeof(head));
+  head.nv = nv;
+  Ctx base;
+  memset(&base, 0, sizeof(base));
+  base.h = &head;
+  int ok = 0;
+  auto run = [&](auto tag) {
+    constexpr int V = decltype(tag)::value;
+    ok = 1;
+    warp_call(base, [&](const Ctx& c) { spd_solve<V>(c, A, dadd, hh, x, scratchH); });
+  };
+  switch (nvp) {
+#if defined(B200_WIDE)
+    case 36: run(std::integral_constant<int, 36>()); break;
+#elif defined(B200_KITCHEN)
+    case 31: run(std::integral_constant<int, 31>()); break;
+#else
+    case 14: run(std::integral_constant<int, 14>()); break;
+    case 15: run(std::integral_constant<int, 15>()); break;
+    case 21: run(std::integral_constant<int, 21>()); break;
+    case 22: run(std::integral_constant<int, 22>()); break;
+    case 30: run(std::integral_constant<int, 30>()); break;
+    case 32: run(std::integral_constant<int, 32>()); break;
+#endif
+    default: break;
+  }
+  return ok ? 0 : -1;
 }
 }
 // in-kernel reset sampling (csrc/reset_sample.cuh), the same code the CUDA reset kernel runs
