@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200SIM_LIB") or os.path.join(_HERE, "libb200sim.so")
 _LIB = None
 
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-DB200_BLOCK_ALIGN", "-DB200_CHOL_SMEM",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
               "-prec-div=false", "-prec-sqrt=false"] + \
     os.environ.get("B200SIM_NVCC_EXTRA", "").split()
 

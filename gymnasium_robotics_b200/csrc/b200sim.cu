@@ -118,35 +118,20 @@ __global__ void reach_reset_kernel(b200sim_reach_reset_t p, unsigned long long s
 #define B200_FOR_ALL_VARIANTS(X) X(7, 14) X(7, 15) X(7, 21) X(14, 14) X(14, 15) X(14, 21) X(28, 14) X(28, 15) X(28, 21) \
   X(7, 22) X(14, 22) X(28, 22) X(7, 30) X(14, 30) X(8, 14) X(8, 15) X(8, 21) X(8, 22) X(16, 14) X(16, 15) X(16, 21) X(16, 22) \
   X(32, 14) X(32, 15) X(32, 21) X(32, 22)
+B200_KERNEL_UNIT(kernel_unit_plain, B200_FOR_ALL_VARIANTS)
 
-// wide build (models with 33..40 dofs), compiled from b200sim_wide.cu with 64-bit dof masks
-extern "C" int b200sim_wide_setattr(int wpb, int smem_bytes);
-extern "C" int b200sim_wide_launch(int wpb, int blocks, size_t smem_bytes, void* stream, const uint32_t* model_dev, const FetchTask* task,
-                                   int mode, int nraw, int N, const StepIO* io);
+// wide build (models with 33..36 dofs), compiled from b200sim_wide.cu with 64-bit dof masks
+extern const KernelUnit kernel_unit_wide;
 #define B200_WIDE_NVP 36
-// build for models with joint equalities / condim 6 (Franka Kitchen), compiled from b200sim_kitchen.cu (flat broad-phase scan) and
-// b200sim_kitchen_groups.cu (two-level broad phase; the default, B200SIM_KITCHEN_GROUPS=0 selects the flat scan)
-extern "C" int b200sim_kitchen_build(const b200_model_view* view, const double* eq_data, const float* ref, int penv_body,
-                                     std::vector<uint32_t>* buf, std::string* err);
-extern "C" int b200sim_kitchen_setattr(int wpb, int smem_bytes);
-extern "C" int b200sim_kitchen_groups_build(const b200_model_view* view, const double* eq_data, const float* ref, int penv_body,
-                                            std::vector<uint32_t>* buf, std::string* err);
-extern "C" int b200sim_kitchen_groups_setattr(int wpb, int smem_bytes);
-extern "C" int b200sim_kitchen_groups_launch(int wpb, int blocks, size_t smem_bytes, void* stream, const uint32_t* model_dev, const FetchTask* task,
-                                             int mode, int nraw, int N, const StepIO* io);
-// b200sim_kitchen_hull.cu: the groups build + support-map narrow phase for MESH geoms (models compiled with mesh_hull)
-extern "C" int b200sim_kitchen_hull_build(const b200_model_view* view, const double* eq_data, const float* ref, int penv_body,
-                                          std::vector<uint32_t>* buf, std::string* err);
-extern "C" int b200sim_kitchen_hull_setattr(int wpb, int smem_bytes);
-extern "C" int b200sim_kitchen_hull_launch(int wpb, int blocks, size_t smem_bytes, void* stream, const uint32_t* model_dev, const FetchTask* task,
-                                             int mode, int nraw, int N, const StepIO* io);
-extern "C" int b200sim_kitchen_launch(int wpb, int blocks, size_t smem_bytes, void* stream, const uint32_t* model_dev, const FetchTask* task,
-                                      int mode, int nraw, int N, const StepIO* io);
-#define B200_KITCHEN_NVP 31   // the kitchen translation unit instantiates NVP = 31 (identity-padded; distinct kernel symbols)
+// builds for models with joint equalities / condim 6 (Franka Kitchen): b200sim_kitchen.cu (flat broad-phase scan),
+// b200sim_kitchen_groups.cu (two-level broad phase; the default, B200SIM_KITCHEN_GROUPS=0 selects the flat scan) and
+// b200sim_kitchen_hull.cu (the groups build + support-map narrow phase for MESH geoms, models compiled with mesh_hull)
+extern const KernelUnit kernel_unit_kitchen, kernel_unit_kitchen_groups, kernel_unit_kitchen_hull;
+#define B200_KITCHEN_NVP 31   // the kitchen translation units instantiate NVP = 31 (identity-padded; distinct kernel symbols)
 
 struct b200sim {
   int N = 0, device = 0;
-  bool kitchen = false, kitchen_groups = false, hull = false;
+  const KernelUnit* unit = nullptr;              // the translation unit whose kernels step this model
   std::vector<uint8_t> blob;
   b200_model_view view;
   std::vector<uint32_t> model_host;
@@ -209,24 +194,20 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   float r[3] = {0, 0, 0};
   if (ref) { r[0] = ref[0]; r[1] = ref[1]; r[2] = ref[2]; }
   std::string err;
-  {
-    // models with joint equalities or condim-6 pairs go to the bring-up translation unit (its contact records are larger)
-    const b200_model_view& v = h->view;
-    for (int e = 0; e < v.neq; e++) if (v.eq_type[e] == B200_EQ_JOINT) h->kitchen = true;
-    for (int p = 0; p < v.npair; p++) if (v.pair_condim[p] == 6) h->kitchen = true;
-  }
+  // models with joint equalities or condim-6 pairs go to a kitchen translation unit (its contact records are larger).  MESH geoms (a
+  // model compiled with mesh_hull: hull vertex tables instead of box proxies) exist in the hull build only; that build is the kitchen
+  // groups build plus the support-map narrow phase, so it serves any model the kitchen build serves
+  const b200_model_view& v = h->view;
+  bool kitchen = false, hull = false;
+  for (int e = 0; e < v.neq; e++) if (v.eq_type[e] == B200_EQ_JOINT) kitchen = true;
+  for (int p = 0; p < v.npair; p++) if (v.pair_condim[p] == 6) kitchen = true;
+  for (int g = 0; g < v.ngeom; g++) if (v.geom_type[g] == B200_GEOM_MESH) hull = kitchen = true;
+  const char* groups = getenv("B200SIM_KITCHEN_GROUPS");   // default: two-level broad phase
+  h->unit = hull ? &kernel_unit_kitchen_hull
+                 : kitchen ? (groups && groups[0] && atoi(groups) == 0 ? &kernel_unit_kitchen : &kernel_unit_kitchen_groups)
+                           : (v.nv > 32 ? &kernel_unit_wide : &kernel_unit_plain);
   const int penv = TASK_IS_ADROIT(task->kind) ? task->penv_body : -1;
-  if (h->kitchen) { const char* g = getenv("B200SIM_KITCHEN_GROUPS"); h->kitchen_groups = !(g && g[0] && atoi(g) == 0); }  // default: two-level broad phase
-  // MESH geoms (a model compiled with mesh_hull: hull vertex tables instead of box proxies) exist in the hull build only; that build
-  // is the kitchen groups build plus the support-map narrow phase, so it serves any model the kitchen build serves
-  for (int g = 0; g < h->view.ngeom; g++) if (h->view.geom_type[g] == B200_GEOM_MESH) h->hull = true;
-  if (h->hull) { h->kitchen = true; h->kitchen_groups = true; }
-  if ((h->kitchen ? (h->hull ? b200sim_kitchen_hull_build(&h->view, eq_data, r, penv, &h->model_host, &err)
-                             : (h->kitchen_groups ? b200sim_kitchen_groups_build(&h->view, eq_data, r, penv, &h->model_host, &err)
-                                                  : b200sim_kitchen_build(&h->view, eq_data, r, penv, &h->model_host, &err)))
-                  : dm_build(h->view, eq_data, r, h->model_host, err, penv)) != 0) {
-    delete h; return fail(nullptr, "b200sim_create: " + err, -4);
-  }
+  if (h->unit->build(v, eq_data, r, penv, h->model_host, err) != 0) { delete h; return fail(nullptr, "b200sim_create: " + err, -4); }
   const DMHead* dh = (const DMHead*)h->model_host.data();
   FetchTask& t = h->task;
   memset(&t, 0, sizeof(t));
@@ -268,8 +249,8 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
     if (!ok) { delete h; return fail(nullptr, "b200sim_create: inconsistent AdroitHandRelocate task", -6); }
   }
   if (t.kind == TASK_KITCHEN) {
-    if (!(h->kitchen && t.nact == dh->nu && t.ngoal == dh->nq && t.nobs == dh->nq + dh->nv)) { delete h; return fail(nullptr, "b200sim_create: inconsistent FrankaKitchen task", -6); }
-  } else if (h->kitchen) { delete h; return fail(nullptr, "b200sim_create: this model needs the kitchen task kind (8)", -6); }
+    if (!(kitchen && t.nact == dh->nu && t.ngoal == dh->nq && t.nobs == dh->nq + dh->nv)) { delete h; return fail(nullptr, "b200sim_create: inconsistent FrankaKitchen task", -6); }
+  } else if (kitchen) { delete h; return fail(nullptr, "b200sim_create: this model needs the kitchen task kind (8)", -6); }
   if (t.kind != TASK_FETCH && t.kind != TASK_ANTMAZE && t.kind != TASK_HAND && t.kind != TASK_HAND_REACH && !TASK_IS_ADROIT(t.kind) && t.kind != TASK_KITCHEN) { delete h; return fail(nullptr, "b200sim_create: unknown task kind", -6); }
   if (t.kind == TASK_HAND && (t.nact != dh->nu || t.ngoal != 7 || t.obj_qadr != dh->nq - 7 || t.obj_dadr != dh->nv - 6 ||
                               t.touch_mode < 0 || t.touch_mode > 3 || (t.touch_mode && dh->nsensor == 0) ||
@@ -298,28 +279,21 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   if (dh->nv <= 21 && (dh->nten > 0 || dh->nfric > 0 || dh->nsensor > 0 || dh->any_round_pair)) h->nvp = 30;  // hand features live in the NVP = 30 build
   // the line search keeps the env's constraint edges in registers: refuse a model with more edge slots than its kernel build holds
   // (the kitchen builds check their own capacity in dm_build)
-  if (!h->kitchen && dm_ls_edges(*dh) > 32 * DM_LS_E(h->nvp)) {
+  if (!kitchen && dm_ls_edges(*dh) > 32 * DM_LS_E(h->nvp)) {
     std::string m = "b200sim_create: the line search of the NVP = " + std::to_string(h->nvp) + " kernel build holds " + std::to_string(32 * DM_LS_E(h->nvp)) +
                     " constraint edges per env, this model needs up to " + std::to_string(dm_ls_edges(*dh));
     delete h; return fail(nullptr, m, -8);
   }
   auto fits = [&](int w) { return ((size_t)dh->hot_words + (size_t)w * dh->scr_words) * 4 + 64 <= 232448; };
-  auto built = [&](int w) {   // an instantiation <w, nvp> exists (the wide ones: b200sim_wide.cu)
-    if (h->nvp == B200_WIDE_NVP) return w == 7 || w == 10 || w == 13 || w == 14;
-    bool b = false;
-#define B200_HAS(W, V) b = b || (w == W && h->nvp == V);
-    B200_FOR_ALL_VARIANTS(B200_HAS)
-#undef B200_HAS
-    return b;
-  };
+  auto built = [&](int w) { return h->unit->has(w, h->nvp); };
   const char* ov = getenv("B200SIM_WPB");   // experiments: a block size that has no instantiation for this build is an error, not a no-op
   const int ovw = ov ? atoi(ov) : 0;
-  if (h->kitchen) {
+  if (kitchen) {
     if (dh->nv > 31) { delete h; return fail(nullptr, "b200sim_create: the kitchen build is instantiated for nv <= 31", -8); }
     h->nvp = B200_KITCHEN_NVP;
-    h->wpb = (num_envs + nsm - 1) / nsm <= 7 ? 7 : ((h->kitchen_groups && fits(11)) ? 11 : (fits(10) ? 10 : 7));
+    h->wpb = (num_envs + nsm - 1) / nsm <= 7 ? 7 : ((built(11) && fits(11)) ? 11 : (fits(10) ? 10 : 7));
     if (ov) {
-      if (!((ovw == 7 || ovw == 10 || (ovw == 11 && h->kitchen_groups)) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no kitchen kernel variant that fits", -8); }
+      if (!(built(ovw) && fits(ovw))) { delete h; return fail(nullptr, "b200sim_create: B200SIM_WPB names no kitchen kernel variant that fits", -8); }
       h->wpb = ovw;
     }
   } else {
@@ -341,12 +315,7 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   h->smem_bytes = ((size_t)dh->hot_words + (size_t)h->wpb * dh->scr_words) * 4;
   h->blocks = (num_envs + h->wpb - 1) / h->wpb;
   h->packed_w = (t.nobs + 2 * t.ngoal + 4 + 3) & ~3;
-  cudaError_t e = cudaErrorInvalidValue;   // stays an error when no instantiation matches (wpb, nvp)
-#define B200_SETATTR(W, V) if (h->wpb == W && h->nvp == V) e = cudaFuncSetAttribute(fetch_kernel<W, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_bytes);
-  B200_FOR_ALL_VARIANTS(B200_SETATTR)
-#undef B200_SETATTR
-  if (h->nvp == B200_WIDE_NVP) e = b200sim_wide_setattr(h->wpb, (int)h->smem_bytes) == 0 ? cudaSuccess : cudaErrorInvalidValue;
-  if (h->nvp == B200_KITCHEN_NVP) e = (h->hull ? b200sim_kitchen_hull_setattr(h->wpb, (int)h->smem_bytes) : (h->kitchen_groups ? b200sim_kitchen_groups_setattr(h->wpb, (int)h->smem_bytes) : b200sim_kitchen_setattr(h->wpb, (int)h->smem_bytes))) == 0 ? cudaSuccess : cudaErrorInvalidValue;
+  const cudaError_t e = h->unit->setattr(h->wpb, h->nvp, (int)h->smem_bytes);
   if (e != cudaSuccess) { std::string m = std::string("b200sim_create: no kernel variant <") + std::to_string(h->wpb) + ", " + std::to_string(h->nvp) + "> or cudaFuncSetAttribute(smem=" + std::to_string(h->smem_bytes) + ") failed: " + cudaGetErrorString(e); delete h; return fail(nullptr, m, -8); }
   const size_t state_bytes = (size_t)num_envs * t.st_stride * 4;
   if (cudaMalloc(&h->model_dev, h->model_host.size() * 4) != cudaSuccess || cudaMalloc(&h->state, state_bytes) != cudaSuccess ||
@@ -414,20 +383,8 @@ static int launch(b200sim* h, int mode, int nraw, const float* actions, const un
   io.terminated = terminated; io.truncated = truncated; io.info = info;
   io.elapsed = h->elapsed; io.max_steps = h->max_steps; io.term_on_success = h->term_on_success; io.overflow_count = h->overflow_count;
   ON_DEVICE(h);
-  int matched = 0;
-#define B200_LAUNCH(W, V)                                                                                   \
-  if (h->wpb == W && h->nvp == V) {                                                                         \
-    matched = 1;                                                                                            \
-    fetch_kernel<W, V><<<h->blocks, W * 32, h->smem_bytes, (cudaStream_t)stream>>>(h->model_dev, h->task, mode, nraw, h->N, io); \
-  }
-  B200_FOR_ALL_VARIANTS(B200_LAUNCH)
-#undef B200_LAUNCH
-  if (h->nvp == B200_KITCHEN_NVP)
-    matched = (h->hull ? b200sim_kitchen_hull_launch : (h->kitchen_groups ? b200sim_kitchen_groups_launch : b200sim_kitchen_launch))(h->wpb, h->blocks, h->smem_bytes, stream, h->model_dev,
-                                                                                        &h->task, mode, nraw, h->N, &io) == 0;
-  if (h->nvp == B200_WIDE_NVP)
-    matched = b200sim_wide_launch(h->wpb, h->blocks, h->smem_bytes, stream, h->model_dev, &h->task, mode, nraw, h->N, &io) == 0;
-  if (!matched) return fail(h, "no kernel variant for this (envs per block, nv) pair: nothing was launched", -8);
+  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io))
+    return fail(h, "no kernel variant for this (envs per block, nv) pair: nothing was launched", -8);
   h->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -8,21 +8,4 @@
 #include "step_kernel.cuh"
 
 #define B200_WIDE_VARIANTS(X) X(7, 36) X(10, 36) X(13, 36) X(14, 36)
-
-extern "C" int b200sim_wide_setattr(int wpb, int smem_bytes) {
-  cudaError_t e = cudaErrorInvalidValue;
-#define B200_SETATTR(W, V) if (wpb == W) e = cudaFuncSetAttribute(fetch_kernel<W, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-  B200_WIDE_VARIANTS(B200_SETATTR)
-#undef B200_SETATTR
-  return e == cudaSuccess ? 0 : -1;
-}
-
-extern "C" int b200sim_wide_launch(int wpb, int blocks, size_t smem_bytes, void* stream, const uint32_t* model_dev, const FetchTask* task,
-                                   int mode, int nraw, int N, const StepIO* io) {
-  int matched = 0;
-#define B200_LAUNCH(W, V)                                                                                        \
-  if (wpb == W) { matched = 1; fetch_kernel<W, V><<<blocks, W * 32, smem_bytes, (cudaStream_t)stream>>>(model_dev, *task, mode, nraw, N, *io); }
-  B200_WIDE_VARIANTS(B200_LAUNCH)
-#undef B200_LAUNCH
-  return matched ? 0 : -1;
-}
+B200_KERNEL_UNIT(kernel_unit_wide, B200_WIDE_VARIANTS)

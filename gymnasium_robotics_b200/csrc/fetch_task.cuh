@@ -559,7 +559,6 @@ template <int NVP, bool REBUILD = false>
 HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, int nraw, float* st, const float* action, float* obs,
                        float* achieved, float* desired, float* reward, float* success, int* iters_out) {
   const DMHead* h = c.h;
-  constexpr int kAlign = ALIGN_LEVEL_FOR(NVP);
   if (active) {
     load_state(c, t, st);
     if (NVP >= 30 && mode == MODE_STEP && (t.kind == TASK_HAND || t.kind == TASK_HAND_REACH || TASK_IS_ADROIT(t.kind))) {
@@ -596,12 +595,11 @@ HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, 
   }
   int nsub = mode == MODE_STEP ? t.n_substeps : (mode == MODE_RAW ? nraw : 0);
   for (int s = 0; s < nsub; s++) {
-    bool solved = false;
-    forward<NVP, REBUILD>(c, active, h->integrator == B200_INT_RK4 ? nullptr : &solved);
+    forward<NVP, REBUILD>(c, active);
     TIC();
-    ALIGN_AT(4); TOC(TM_BARRIER);
+    if (NVP >= 30) ALIGN(); TOC(TM_BARRIER);
     if (h->integrator == B200_INT_RK4) rk4_substep<NVP, REBUILD>(c, active);
-    else if (active) euler_step<NVP>(stage_ctx<REBUILD>(c), solved);
+    else if (active) euler_step<NVP>(stage_ctx<REBUILD>(c));
     TOC(TM_INTEG);
   }
   // touch sensors read the contacts and forces of the last forward pass: a refresh (no sub-step) runs one first,

@@ -29,40 +29,8 @@
 #define WARP_W 32
 #define SYNC() __syncwarp()
 // block-wide alignment points: keep the warps of a block inside the same code window (instruction-cache locality)
-#ifdef B200_BLOCK_ALIGN
-// the alignment group is the whole block
-#ifdef B200_ALIGN_SYNCWARP
-#define ALIGN() do { __syncwarp(); __syncthreads(); } while (0)
-#define ALIGN_OR(p) (__syncwarp(), __syncthreads_or(p))
-#elif defined(B200_AG)
-// A/B variant: alignment groups of B200_AG warps inside the block (named barriers 1 + group): fewer warps wait for one straggler, at the
-// price of as many code windows per SM as there are groups
-static __device__ __forceinline__ void b200_bar_g(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-static __device__ __forceinline__ bool b200_bar_or_g(int id, int nthreads, bool p) {
-  int r;
-  asm volatile("{ .reg .pred q, r; setp.ne.s32 q, %3, 0; bar.red.or.pred r, %1, %2, q; selp.s32 %0, 1, 0, r; }" : "=r"(r) : "r"(id), "r"(nthreads), "r"((int)p) : "memory");
-  return r != 0;
-}
-#define ALIGN() b200_bar_g(1 + (int)(threadIdx.x >> 5) / B200_AG, B200_AG * 32)
-#define ALIGN_OR(p) b200_bar_or_g(1 + (int)(threadIdx.x >> 5) / B200_AG, B200_AG * 32, (p))
-#elif defined(B200_ALIGN_NONALIGNED)
-// A/B variant: PTX `barrier.sync` WITHOUT `.aligned` -- the form that tolerates a warp arriving in several convergence groups
-static __device__ __forceinline__ void b200_bar_na() { asm volatile("barrier.sync 0;" ::: "memory"); }
-static __device__ __forceinline__ bool b200_bar_or_na(bool p) {
-  int r;
-  asm volatile("{ .reg .pred q, r; setp.ne.s32 q, %1, 0; barrier.red.or.pred r, 0, q; selp.s32 %0, 1, 0, r; }" : "=r"(r) : "r"((int)p) : "memory");
-  return r != 0;
-}
-#define ALIGN() b200_bar_na()
-#define ALIGN_OR(p) b200_bar_or_na(p)
-#else
 #define ALIGN() __syncthreads()
 #define ALIGN_OR(p) __syncthreads_or(p)
-#endif
-#else
-#define ALIGN() do { } while (0)
-#define ALIGN_OR(p) (p)
-#endif
 #elif defined(B200_HOST_WARP)
 #define HD static inline
 #define HDN static
@@ -87,16 +55,6 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #endif
 
-// Address-space hint for the narrow-phase lane slots.  Observed on the GPU: with the hint on the slot
-// reference inside collision() the kernel reads garbage addresses (compute-sanitizer: invalid __shared__ read in the NEXT broad
-// phase; the 32-lane host emulation under ASan / UBSan is clean, the same build without the hint is clean on the GPU) -- the
-// slot address is a per-lane select between two scratch regions and nvcc 12.9 mis-handles the assumption there.  collision()
-// therefore reaches its slot through generic loads / stores; the hint inside the callees is opt-in (-DB200_SLOT_ASSUME).
-#ifdef B200_SLOT_ASSUME
-#define ASSUME_SHARED_SLOT(p) ASSUME_SHARED_PTR(p)
-#else
-#define ASSUME_SHARED_SLOT(p) do { } while (0)
-#endif
 #define B200_MINVAL 1e-15f
 #define B200_MINIMP 0.0001f
 #define B200_MAXIMP 0.9999f
@@ -646,7 +604,6 @@ HD void collide_plane_box(const Ctx& c, int g1, int g2, float margin, ContactOut
 }
 
 HD int clip_poly(const float (*in)[2], int n, float (*out)[2], int axis, float bound, float sign) {
-  ASSUME_SHARED_SLOT(in); ASSUME_SHARED_SLOT(out);
   int k = 0;
   for (int i = 0; i < n; i++) {
     const float* a = in[i];
@@ -663,7 +620,6 @@ HD int clip_poly(const float (*in)[2], int n, float (*out)[2], int axis, float b
 
 HDN void collide_box_box(const Ctx c, int g1, int g2, float margin, ContactOut& o, BoxScratch& bs) {
   ASSUME_SHARED(c);
-  ASSUME_SHARED_SLOT(&bs);
   float pa[3], Ra[9], pb[3], Rb[9];
   geom_pose(c, g1, pa, Ra); geom_pose(c, g2, pb, Rb);
   const float* ha = MF(geom_size) + 3 * g1;
@@ -1352,6 +1308,8 @@ STAGE void collision(const Ctx c) {
   // round: every working lane owns a BoxScratch slot in shared memory (the result record itself stays on the lane's stack)
   int ncand = cnt[CNT_NCAND];
   const int nslotA = h->ncslotA, nslotAB = nslotA + h->ncslotB;
+  // no __isShared assumption on this per-lane select between two scratch regions: with one, nvcc 12.9 miscompiled the kernel
+  // (invalid __shared__ reads in the next broad phase on the GPU)
   BoxScratch& bs = *(BoxScratch*)(c.lane < nslotA ? c.s + h->s_cslotA + c.lane * DM_CSLOT_WORDS
                                                   : c.s + h->s_cslotB + ((c.lane < nslotAB ? c.lane : nslotA) - nslotA) * DM_CSLOT_WORDS);
   for (int base = 0, nslot = 0; base < ncand; base += nslot) {
@@ -2105,14 +2063,12 @@ static __device__ __noinline__ void spd_solve(const Ctx c, const float* A, const
   float b = 0.f;
   if (live) b = x[i];  // predicated load: idle lanes never touch x
   float dinv = 1.f;
-#ifdef B200_CHOL_SMEM
   // column k of L travels through shared memory (one store per lane, 128-bit broadcast loads) instead of one shuffle per
   // (row, column) pair; two alternating buffers in the dead `scratchH` region (A has been loaded into registers above;
   // when A == scratchH the warp-level barrier below orders the overwrite)
   constexpr int NA4 = (NA + 3) & ~3;
   float* colbuf = scratchH;
   __syncwarp();
-#endif
 #pragma unroll
   for (int k = 0; k < NA; k++) {
     float hkk = __shfl_sync(FULL, h[k], k);
@@ -2120,7 +2076,6 @@ static __device__ __noinline__ void spd_solve(const Ctx c, const float* A, const
     float lik = (i > k) ? h[k] * inv : 0.f;
     dinv = (i == k) ? inv : dinv;
     h[k] = (i > k) ? lik : h[k];
-#ifdef B200_CHOL_SMEM
     if (k + 1 < NA) {
       float* col = colbuf + (k & 1) * NA4;
       if (i < NA4) col[i] = lik;
@@ -2135,10 +2090,6 @@ static __device__ __noinline__ void spd_solve(const Ctx c, const float* A, const
         if (4 * q + 3 > k && 4 * q + 3 < NA) h[4 * q + 3] = fmaf(-lik, v.w, h[4 * q + 3]);
       }
     }
-#else
-#pragma unroll
-    for (int j = k + 1; j < NA; j++) { float ljk = __shfl_sync(FULL, lik, j); h[j] = fmaf(-lik, ljk, h[j]); }
-#endif
     float lr[KS];
 #pragma unroll
     for (int r = 0; r < KB; r++) {
@@ -2438,9 +2389,6 @@ STAGE int newton_check(const Ctx c, int iter, float improvement) {
   }
   SYNC();
   float gnorm = sqrtf(wsum(g2sum)), fnorm = sqrtf(wsum(f2sum));
-#if defined(B200_DEBUG_SOLVER) && !defined(__CUDACC__)
-  printf("  iter %d gnorm %.3e fnorm %.3e improvement %.3e\n", iter, gnorm, fnorm, improvement);
-#endif
   // single-precision floor: the gradient cannot be resolved below ~eps32 * (|M a| + |f_smooth| + |f_constraint|)
   if (gnorm < 2e-6f * fnorm) return 1;
   if (iter > 0 && (scale * improvement < tol || scale * gnorm < tol)) return 1;
@@ -2510,69 +2458,41 @@ STAGE void euler_solve(const Ctx c) {
 // One forward pass.  `active` is warp-uniform; idle warps (no env, or masked out) only take part in the block-wide
 // alignment barriers, so every warp of the block executes the same barrier sequence.  The Newton loop runs until every
 // warp of the block has converged (converged warps idle through the remaining rounds).
-#ifndef B200_ALIGN_LEVEL
-#define B200_ALIGN_LEVEL 3
-#endif
-// alignment density per kernel build: the hand build (NVP = 30, 14 warps per block) gains from the finest level
-#define ALIGN_LEVEL_FOR(NVP) ((NVP) >= 30 ? 4 : B200_ALIGN_LEVEL)
-#define ALIGN_AT(level) do { if (kAlign >= (level)) ALIGN(); } while (0)
-// `euler_solved` (optional): the caller integrates with the implicit-damping Euler step right after this pass.  A warp whose
-// Newton solve has converged then runs the (M + h B) solve of that step while the other warps of the block run their next
-// Newton direction solve -- the same routine (spd_solve<NVP>), i.e. the same code window -- instead of idling at the barrier;
-// *euler_solved tells euler_step that SF(search) already holds the solution.
 template <int NVP, bool REBUILD = false>
-HD void forward(const Ctx c, bool active, bool* euler_solved = nullptr) {
+HD void forward(const Ctx c, bool active) {
   constexpr bool HF = NVP >= 30;
   constexpr bool CX = NVP == 22 || NVP >= 30;   // NVP 22 = the 21-dof arm build plus the convex collider (FetchSlide)
-  constexpr int kAlign = ALIGN_LEVEL_FOR(NVP);
   constexpr int kLsE = DM_LS_E(NVP);   // line-search edge slots per lane
+  // HF: the hand build (NVP >= 30, 14 warps per block) is faster with a barrier after every stage (DESIGN.md 3, "Hand build")
   TIC();
-#ifndef B200_NO_ALIGN_FIRST
-  ALIGN_AT(1); TOC(TM_BARRIER);
-#endif
+  ALIGN(); TOC(TM_BARRIER);
   if (active) kinematics(stage_ctx<REBUILD>(c));
-  TOC(TM_KIN); ALIGN_AT(4); TOC(TM_BARRIER);
+  TOC(TM_KIN); if (HF) ALIGN(); TOC(TM_BARRIER);
   if (active) { com_quantities(stage_ctx<REBUILD>(c)); mass_matrix(stage_ctx<REBUILD>(c)); }
-#ifndef B200_NO_ALIGN_PRECOLL
-  TOC(TM_COM_M); ALIGN_AT(2); TOC(TM_BARRIER);
-#endif
+  TOC(TM_COM_M); ALIGN(); TOC(TM_BARRIER);
   if (active) collision<HF, CX>(stage_ctx<REBUILD>(c));
-  TOC(TM_COLL); ALIGN_AT(2); TOC(TM_BARRIER);
+  TOC(TM_COLL); ALIGN(); TOC(TM_BARRIER);
   if (active) make_constraint<HF>(stage_ctx<REBUILD>(c));
-  TOC(TM_CONSTR); ALIGN_AT(4); TOC(TM_BARRIER);
+  TOC(TM_CONSTR); if (HF) ALIGN(); TOC(TM_BARRIER);
   if (active) smooth_forces(stage_ctx<REBUILD>(c));
-  TOC(TM_SMOOTH); ALIGN_AT(4); TOC(TM_BARRIER);
+  TOC(TM_SMOOTH); if (HF) ALIGN(); TOC(TM_BARRIER);
   if (active) newton_begin<HF>(stage_ctx<REBUILD>(c));
   TOC(TM_NBEGIN);
   int done = active ? 0 : 1;
   float improvement = 0;
-  if (kAlign >= 3) {
-    for (int iter = 0;; iter++) {
-      ALIGN(); TOC(TM_BARRIER);
-      if (!done) done = newton_check<HF>(stage_ctx<REBUILD>(c), iter, improvement);
-      TOC(TM_NCHECK);
-      bool more = ALIGN_OR(!done);
-      TOC(TM_BARRIER);
-      if (!more) break;
-      if (!done) build_H<HF>(stage_ctx<REBUILD>(c));
-      TOC(TM_BUILDH); ALIGN_AT(4); TOC(TM_BARRIER);
-      if (!done) newton_direction<NVP>(stage_ctx<REBUILD>(c));
-#ifdef B200_EULER_PIGGYBACK
-      else if (euler_solved && active && !*euler_solved && c.h->any_damping) { euler_solve<NVP>(stage_ctx<REBUILD>(c)); *euler_solved = true; }
-#endif
-      TOC(TM_NDIR); ALIGN(); TOC(TM_BARRIER);
-      if (!done) done = newton_move<HF, kLsE>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
-      TOC(TM_NMOVE);
-    }
-  } else {
-    ALIGN_AT(2);
-    for (int iter = 0; !done; iter++) {
-      done = newton_check<HF>(c, iter, improvement);
-      if (done) break;
-      build_H<HF>(c);
-      newton_direction<NVP>(c);
-      done = newton_move<HF, kLsE>(c, &improvement) ? 2 : 0;
-    }
+  for (int iter = 0;; iter++) {
+    ALIGN(); TOC(TM_BARRIER);
+    if (!done) done = newton_check<HF>(stage_ctx<REBUILD>(c), iter, improvement);
+    TOC(TM_NCHECK);
+    bool more = ALIGN_OR(!done);
+    TOC(TM_BARRIER);
+    if (!more) break;
+    if (!done) build_H<HF>(stage_ctx<REBUILD>(c));
+    TOC(TM_BUILDH); if (HF) ALIGN(); TOC(TM_BARRIER);
+    if (!done) newton_direction<NVP>(stage_ctx<REBUILD>(c));
+    TOC(TM_NDIR); ALIGN(); TOC(TM_BARRIER);
+    if (!done) done = newton_move<HF, kLsE>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
+    TOC(TM_NMOVE);
   }
 }
 
@@ -2602,14 +2522,14 @@ STAGE void integrate_pos(const Ctx c, float* qpos, const float* qvel, float hh) 
 }
 
 template <int NVP>
-STAGE void euler_step(const Ctx c, bool solved = false) {
+STAGE void euler_step(const Ctx c) {
   ASSUME_SHARED(c);
   const DMHead* h = c.h;
   int nv = h->nv;
   float hh = h->timestep;
   float* x = SF(search);  // qacc itself is next sub-step's warm start
   if (h->any_damping) {
-    if (!solved) euler_solve<NVP>(c);
+    euler_solve<NVP>(c);
   } else {
     LANES(i, nv) x[i] = SF(qacc)[i];
     SYNC();

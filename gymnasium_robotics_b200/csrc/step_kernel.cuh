@@ -1,6 +1,7 @@
 // The step kernel: one warp integrates one env for a whole env-step (all sub-steps on chip); WPB warps share one copy of
 // the model constants that a single thread stages into shared memory with a TMA bulk copy (cp.async.bulk + mbarrier).
-// Included by b200sim.cu (32-bit dof masks, NVP <= 30) and by b200sim_wide.cu (B200_WIDE: 64-bit dof masks, NVP = 36).
+// Included by each kernel build (translation unit): b200sim.cu (32-bit dof masks, NVP <= 30), b200sim_wide.cu (B200_WIDE: 64-bit
+// dof masks, NVP = 36) and the three b200sim_kitchen*.cu; each one names its instantiations once, in B200_KERNEL_UNIT.
 #pragma once
 #include <cuda_runtime.h>
 #include "fetch_task.cuh"
@@ -100,3 +101,40 @@ __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restr
 #endif
 }
 
+// One kernel build: its model builder (the scratch layout depends on the unit's defines) and its fetch_kernel<WPB, NVP>
+// instantiations.  b200sim_create picks the unit of a model once and keeps it on the handle.
+struct KernelUnit {
+  int (*build)(const b200_model_view& view, const double* eq_data, const float* ref, int penv_body, std::vector<uint32_t>& buf,
+               std::string& err);
+  bool (*has)(int wpb, int nvp);                                // an instantiation <wpb, nvp> exists
+  cudaError_t (*setattr)(int wpb, int nvp, int smem_bytes);     // cudaErrorInvalidValue when it does not
+  bool (*launch)(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev, const FetchTask& task,
+                 int mode, int nraw, int N, const StepIO& io);  // false (nothing launched) when it does not
+};
+
+#define B200_UNIT_HAS(W, V) || (wpb == W && nvp == V)
+#define B200_UNIT_SETATTR(W, V) \
+  if (wpb == W && nvp == V) return cudaFuncSetAttribute(fetch_kernel<W, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+#define B200_UNIT_LAUNCH(W, V)                                                                           \
+  if (wpb == W && nvp == V) {                                                                            \
+    fetch_kernel<W, V><<<blocks, W * 32, smem_bytes, stream>>>(model_dev, task, mode, nraw, N, io);      \
+    return true;                                                                                         \
+  }
+
+// Defines `const KernelUnit NAME` from the unit's instantiation list VARIANTS(X): one X(WPB, NVP) per kernel.
+#define B200_KERNEL_UNIT(NAME, VARIANTS)                                                                                              \
+  static int unit_build(const b200_model_view& view, const double* eq_data, const float* ref, int penv_body, std::vector<uint32_t>& buf, \
+                        std::string& err) {                                                                                          \
+    return dm_build(view, eq_data, ref, buf, err, penv_body);                                                                       \
+  }                                                                                                                                  \
+  static bool unit_has(int wpb, int nvp) { return false VARIANTS(B200_UNIT_HAS); }                                                   \
+  static cudaError_t unit_setattr(int wpb, int nvp, int smem_bytes) {                                                                \
+    VARIANTS(B200_UNIT_SETATTR)                                                                                                      \
+    return cudaErrorInvalidValue;                                                                                                    \
+  }                                                                                                                                  \
+  static bool unit_launch(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev,           \
+                          const FetchTask& task, int mode, int nraw, int N, const StepIO& io) {                                      \
+    VARIANTS(B200_UNIT_LAUNCH)                                                                                                       \
+    return false;                                                                                                                    \
+  }                                                                                                                                  \
+  extern const KernelUnit NAME = {unit_build, unit_has, unit_setattr, unit_launch};

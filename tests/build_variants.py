@@ -1,13 +1,17 @@
 """Build library variants for A/B timing on the GPU box (experiments): python tests/build_variants.py name[:srcdir][:extra flags] ...
-Each variant is compiled from `srcdir` (default: this checkout) into build/variants/lib<name>.so.
-The tests/gpu_round*.sh recipes that read an older directory are retired."""
+Each variant is compiled from `srcdir` (default: this checkout) into build/variants/lib<name>.so, with this checkout's library
+nvcc flags.  A `srcdir` from before the experiment-only build knobs were removed needs, among the extra flags, the two defines that
+its own _lib.NVCC_FLAGS carried: without them it compiles without block-wide barriers and with the shuffle Cholesky, which is not
+the library that checkout shipped."""
 import os
 import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BASE = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-DB200_BLOCK_ALIGN",
-        "-DB200_CHOL_SMEM", "-prec-div=false", "-prec-sqrt=false"]
+sys.path.insert(0, ROOT)
+from gymnasium_robotics_b200 import _lib  # noqa: E402
+
+BASE = [f for f in _lib.NVCC_FLAGS if f != "-shared"]
 NAMES = ("b200sim", "b200sim_wide", "b200sim_kitchen", "b200sim_kitchen_groups", "b200sim_kitchen_hull")
 
 

@@ -56,15 +56,15 @@ def build(force=False, wide=False):
                                       ({"kitchen": ["-DB200_KITCHEN"], "kitchen_groups": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS"],
                                         "kitchen_flat": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS", "-DB200_KITCHEN_FLATSCAN"],
                                         # WARP_W == 32 on lock-step fibers (hostwarp.h): the lane-parallel code paths themselves
-                                        "warp": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-Wno-unknown-pragmas"],
-                                        "warp_wide": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-DB200_WIDE", "-Wno-unknown-pragmas"],
-                                        "warp_timing": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-DB200_STAGE_TIMING", "-Wno-unknown-pragmas"],
-                                        "warp_kitchen": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-DB200_KITCHEN", "-Wno-unknown-pragmas"],
-                                        "warp_kitchen_groups": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
+                                        "warp": ["-DB200_HOST_WARP", "-Wno-unknown-pragmas"],
+                                        "warp_wide": ["-DB200_HOST_WARP", "-DB200_WIDE", "-Wno-unknown-pragmas"],
+                                        "warp_timing": ["-DB200_HOST_WARP", "-DB200_STAGE_TIMING", "-Wno-unknown-pragmas"],
+                                        "warp_kitchen": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-Wno-unknown-pragmas"],
+                                        "warp_kitchen_groups": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
                                                                 "-Wno-unknown-pragmas"],
                                         # the kitchen groups build + the support-map narrow phase for mesh geoms (csrc/b200sim_kitchen_hull.cu)
                                         "kitchen_hull": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS", "-DB200_HULL"],
-                                        "warp_kitchen_hull": ["-DB200_HOST_WARP", "-DB200_CHOL_SMEM", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
+                                        "warp_kitchen_hull": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
                                                               "-DB200_HULL", "-Wno-unknown-pragmas"]}.get(wide) or
                                        (["-DB200_WIDE"] if wide else [])) + ["-o", tmp, srcs[0]])
                 os.replace(tmp, out)
