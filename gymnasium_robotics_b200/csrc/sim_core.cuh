@@ -939,7 +939,11 @@ HDN void collide_round_round(const Ctx c, int g1, int g2, float margin, ContactO
   float h1 = MI(geom_type)[g1] == B200_GEOM_CAPSULE ? MF(geom_size)[3 * g1 + 1] : 0.f;
   float h2 = MI(geom_type)[g2] == B200_GEOM_CAPSULE ? MF(geom_size)[3 * g2 + 1] : 0.f;
   float w[3] = {p1[0] - p2[0], p1[1] - p2[1], p1[2] - p2[2]};
-  float b = dot3(a1, a2), d = dot3(a1, w), e = dot3(a2, w), den = 1 - b * b, sp = 0, tp = 0;
+  // den = |a1 x a2|^2 = sin^2 theta: 1 - (a1.a2)^2 cancels to nothing below theta ~ 3e-4 in fp32 and is not sin^2 theta for axes
+  // that are unit only to 1e-7 (identical axes gave den ~ 1e-7, a "non-parallel" solve and a contact millimetres off)
+  float cx[3];
+  cross3(cx, a1, a2);
+  float b = dot3(a1, a2), d = dot3(a1, w), e = dot3(a2, w), den = dot3(cx, cx), sp = 0, tp = 0;
   if (h1 <= 0 && h2 <= 0) { sp = 0; tp = 0; }
   else if (h1 <= 0) { sp = 0; tp = e; }
   else if (h2 <= 0) { tp = 0; sp = -d; }

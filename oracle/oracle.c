@@ -824,7 +824,9 @@ static void collide_capsule_box(oracle_sim* s, int pair, real margin) {
 static void segment_closest(const real* p1, const real* a1, real h1, const real* p2, const real* a2, real h2, real* s_out, real* t_out) {
   real w[3];
   sub3(w, p1, p2);
-  real b = dot3(a1, a2), d = dot3(a1, w), e = dot3(a2, w), den = 1 - b * b, sp, tp;
+  real cx[3];
+  cross3(cx, a1, a2);   /* den = |a1 x a2|^2 = sin^2 theta (not 1 - b^2: no cancellation, and exact for non-unit axes too) */
+  real b = dot3(a1, a2), d = dot3(a1, w), e = dot3(a2, w), den = dot3(cx, cx), sp, tp;
   if (h1 <= 0 && h2 <= 0) { *s_out = 0; *t_out = 0; return; }
   if (h1 <= 0) { sp = 0; tp = e; }
   else if (h2 <= 0) { tp = 0; sp = -d; }
@@ -1854,9 +1856,13 @@ void oracle_cfrc_ext(const oracle_sim* s, real* out) {
   }
 }
 int oracle_cfrc_rows(const oracle_sim* s) { return s->m.n_mjbody_rt > 0 ? s->m.n_mjbody_rt : s->nbody; }
-/* contact k -> out[0]=dist, out[1:4]=pos, out[4:13]=frame, out[13]=dim, out[14]=geom1, out[15]=geom2, out[16]=efc_address */
+/* contact k -> out[0]=dist, out[1:4]=pos, out[4:13]=frame, out[13]=dim, out[14]=geom1, out[15]=geom2, out[16]=efc_address,
+ * out[17]=pair */
 void oracle_contact(const oracle_sim* s, int k, real* out) {
   const Contact* c = &s->con[k];
   out[0] = c->dist; memcpy(out + 1, c->pos, 3 * sizeof(real)); memcpy(out + 4, c->frame, 9 * sizeof(real));
-  out[13] = c->dim; out[14] = c->geom1; out[15] = c->geom2; out[16] = c->efc_address;
+  out[13] = c->dim; out[14] = c->geom1; out[15] = c->geom2; out[16] = c->efc_address; out[17] = c->pair;
 }
+/* the collision stage alone, from the current geom_xpos / geom_xmat (no kinematics): the contact list that contacts() reads.
+ * Tests of the narrow phase set the geom poses directly, so that both sides collide exactly the same inputs. */
+void oracle_collision(oracle_sim* s) { collision(s); }

@@ -60,7 +60,7 @@ def lib():
         L = _load_native() if _NATIVE else ctypes.CDLL(build())
         L.oracle_create.restype = ctypes.c_void_p
         L.oracle_create.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
-        for f in ("oracle_destroy", "oracle_reset_data", "oracle_forward"):
+        for f in ("oracle_destroy", "oracle_reset_data", "oracle_forward", "oracle_collision"):
             getattr(L, f).argtypes = [ctypes.c_void_p]
             getattr(L, f).restype = None
         L.oracle_step.argtypes = [ctypes.c_void_p, ctypes.c_int]
@@ -135,6 +135,10 @@ class OracleSim:
     def forward(self):
         self._L.oracle_forward(self._h)
 
+    def collision(self):
+        """The collision stage alone, from the current geom_xpos / geom_xmat (no kinematics); contacts() reads the result."""
+        self._L.oracle_collision(self._h)
+
     def step(self, nstep=1):
         self._L.oracle_step(self._h, int(nstep))
 
@@ -180,11 +184,11 @@ class OracleSim:
 
     def contacts(self):
         out = []
-        buf = np.zeros(17)
+        buf = np.zeros(18)
         for k in range(self.ncon):
             self._L.oracle_contact(self._h, k, buf.ctypes.data)
             out.append(dict(dist=buf[0], pos=buf[1:4].copy(), frame=buf[4:13].copy().reshape(3, 3), dim=int(buf[13]),
-                            geom1=int(buf[14]), geom2=int(buf[15]), efc_address=int(buf[16])))
+                            geom1=int(buf[14]), geom2=int(buf[15]), efc_address=int(buf[16]), pair=int(buf[17])))
         return out
 
     def efc(self, name):

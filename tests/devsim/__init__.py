@@ -21,8 +21,10 @@ FLAVORS = {
     "plain": ("b200sim.cu", [], (14, 15, 21, 22, 30)),
     "wide": ("b200sim_wide.cu", ["-DB200_WIDE"], (36,)),
     "kitchen": ("b200sim_kitchen.cu", ["-DB200_KITCHEN"], (31,)),
+    "kitchen_groups": ("b200sim_kitchen_groups.cu", ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS"], (31,)),
 }
-NVP_FLAVOR = {v: f for f, (_, _, vs) in FLAVORS.items() for v in vs}
+# the library that runs the register Cholesky of an NVP (the kitchen units share one spd_solve<31>)
+NVP_FLAVOR = {v: f for f, (_, _, vs) in FLAVORS.items() for v in vs if f != "kitchen_groups"}
 
 
 def build(flavor="plain", force=False):
@@ -57,6 +59,18 @@ def lib(flavor="plain"):
         L.devsim_spd.argtypes = [ci, ci, vp, vp, vp, ctypes.c_float, ci, vp, vp, ci, ci, ci, ci]
         L.devsim_spd.restype = ci
         L.devsim_last_error.restype = ctypes.c_char_p
+        L.devsim_model_create.restype = vp
+        L.devsim_model_create.argtypes = [ctypes.c_char_p, ctypes.c_size_t, vp, vp, ci, ci]
+        L.devsim_model_destroy.argtypes = [vp]
+        L.devsim_model_words.restype = ctypes.POINTER(ctypes.c_uint32)
+        L.devsim_model_words.argtypes = [vp]
+        L.devsim_scr_words.argtypes = [vp]
+        L.devsim_model_nwords.argtypes = [vp]
+        L.devsim_layout.argtypes = [vp]
+        L.devsim_layout.restype = None
+        L.devsim_offset.argtypes = [vp, ctypes.c_char_p, ci]
+        L.devsim_stage.argtypes = [vp, ci, ci, ci, vp]
+        L.devsim_stage.restype = ci
         _LIB[flavor] = L
     return _LIB[flavor]
 
@@ -72,3 +86,49 @@ def spd(nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
                       H.ctypes.data, A.shape[1], x.shape[1], H.shape[1], int(bool(inplace)))
     if rc != 0:
         raise RuntimeError(f"devsim_spd(nvp={nvp}): {L.devsim_last_error().decode()}")
+
+
+STAGE_COLLIDE, STAGE_KIN = 0, 1
+LAYOUT = ("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE")
+
+
+class DevModel:
+    """The device model of `model` as the `flavor` unit builds it, and single stages of that unit on batches of scratch images."""
+
+    def __init__(self, flavor, model, eq_data=None, ref=(1.0, 0.75, 0.4), penv_body=-1, ngrp_cap=0):
+        self.flavor, self.model = flavor, model
+        L = self._L = lib(flavor)
+        blob = model.to_blob()
+        eq = np.ascontiguousarray(eq_data, dtype=np.float64) if eq_data is not None else None
+        r = np.asarray(ref, dtype=np.float32)
+        self._h = L.devsim_model_create(blob, len(blob), eq.ctypes.data if eq is not None else None, r.ctypes.data, int(penv_body),
+                                        int(ngrp_cap))
+        if not self._h:
+            raise RuntimeError(f"devsim_model_create({flavor}): {L.devsim_last_error().decode()}")
+        self.scr_words = L.devsim_scr_words(self._h)
+        self.words = np.ctypeslib.as_array(L.devsim_model_words(self._h), shape=(L.devsim_model_nwords(self._h),)).copy()
+        lay = np.zeros(6, np.int32)
+        L.devsim_layout(lay.ctypes.data)
+        self.layout = dict(zip(LAYOUT, lay.tolist()))
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.devsim_model_destroy(self._h)
+            self._h = None
+
+    def offset(self, name):
+        o = self._L.devsim_offset(self._h, name.encode(), 0)
+        assert o >= 0, name
+        return o
+
+    def model_offset(self, name):
+        o = self._L.devsim_offset(self._h, name.encode(), 1)
+        assert o >= 0, name
+        return o
+
+    def run(self, nvp, stage, scratch):
+        """stage (STAGE_COLLIDE / STAGE_KIN) of the NVP = nvp instantiation on scratch images [n, scr_words] float32, in place."""
+        assert scratch.dtype == np.float32 and scratch.flags.c_contiguous and scratch.shape[1] == self.scr_words
+        rc = self._L.devsim_stage(self._h, int(nvp), int(stage), scratch.shape[0], scratch.ctypes.data)
+        if rc != 0:
+            raise RuntimeError(f"devsim_stage({self.flavor}, nvp={nvp}): {self._L.devsim_last_error().decode()}")

@@ -9,12 +9,20 @@
 // spd: spd_solve<NVP>, the register Cholesky of the Newton direction (A == scratchH, in place) and of the implicit-damping Euler
 // step (A = M, dadd = dof damping, scratchH = the dead H region).  Only the header's nv is read, so a zeroed header with nv set
 // stands for the model, and any nv up to NVP can be solved.
+//
+// collide / kin: whole stages on a real model (dm_build on the host with this library's defines), staged as the step kernel
+// stages it (step_kernel.cuh): header + HOT arrays in shared memory, the COLD arrays -- the kitchen groups build's pair list among
+// them -- read from the global model, one env's scratch after the hot words.  The host hands in a whole scratch image per case
+// and gets the whole image back.  collide = collision<HF, CX> with HF and CX derived from NVP as forward<NVP> derives them;
+// kin = kinematics, com_quantities and mass_matrix.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
 
 #include "../../gymnasium_robotics_b200/csrc/fetch_task.cuh"
+#include <string>
+#include <vector>
 
 // header words in front of the operands, rounded to 16 bytes (the register Cholesky reads its column buffers as float4)
 #define DEVSIM_HEAD_WORDS ((int)((sizeof(DMHead) + 15) / 16 * 4))
@@ -108,4 +116,120 @@ extern "C" int devsim_spd(int nvp, int ncase, const int* nv, float* A, const flo
 done:
   cudaFree(d_nv); cudaFree(d_A); cudaFree(d_D); cudaFree(d_x); cudaFree(d_H);
   return rc;
+}
+
+enum { DEVSIM_COLLIDE = 0, DEVSIM_KIN = 1 };
+
+template <int NVP>
+__global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ model, int stage, float* scratch) {
+  const int e = blockIdx.x, lane = threadIdx.x;
+  const DMHead* hg = (const DMHead*)model;
+  const int hot = hg->hot_words, sw = hg->scr_words;
+  for (int k = lane; k < hot; k += 32) b200_smem[k] = model[k];
+  float* s = (float*)(b200_smem + hot);
+  for (int k = lane; k < sw; k += 32) s[k] = scratch[(size_t)e * sw + k];
+  __syncwarp();
+  Ctx c;
+  c.mg = model; c.mw = b200_smem; c.h = (const DMHead*)b200_smem; c.s = s; c.lane = lane;
+#ifdef B200_STAGE_TIMING
+  c.tim = nullptr;
+#endif
+  constexpr bool HF = NVP >= 30;
+  constexpr bool CX = NVP == 22 || NVP >= 30;
+  if (stage == DEVSIM_COLLIDE) collision<HF, CX>(c);
+  else { kinematics(c); com_quantities(c); mass_matrix(c); }
+  __syncwarp();
+  for (int k = lane; k < sw; k += 32) scratch[(size_t)e * sw + k] = s[k];
+}
+
+#ifdef B200_WIDE
+static const bool kWide = true;   // 64-bit dof masks, as hostsim's wide flavor builds them
+#else
+static const bool kWide = false;
+#endif
+
+struct DevModel {
+  std::vector<uint8_t> blob;
+  b200_model_view view;
+  std::vector<uint32_t> model;
+};
+
+extern "C" {
+// the device model of a blob as this library's unit builds it (NULL on a refusal: devsim_last_error())
+void* devsim_model_create(const void* blob, size_t n, const double* eq_data, const float* ref, int penv_body, int ngrp_cap) {
+  DevModel* d = new DevModel;
+  std::string err;
+  d->blob.assign((const uint8_t*)blob, (const uint8_t*)blob + n);
+  if (b200_model_parse(d->blob.data(), n, &d->view) != 0) { snprintf(g_err, sizeof(g_err), "not a model blob"); delete d; return nullptr; }
+  if (dm_build(d->view, eq_data, ref, d->model, err, penv_body, kWide, ngrp_cap) != 0) {
+    snprintf(g_err, sizeof(g_err), "dm_build: %s", err.c_str());
+    delete d;
+    return nullptr;
+  }
+  return d;
+}
+void devsim_model_destroy(void* p) { delete (DevModel*)p; }
+const uint32_t* devsim_model_words(void* p) { return ((DevModel*)p)->model.data(); }
+int devsim_scr_words(void* p) { return ((const DMHead*)((DevModel*)p)->model.data())->scr_words; }
+int devsim_model_nwords(void* p) { return ((const DMHead*)((DevModel*)p)->model.data())->nwords; }
+// this library's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE
+void devsim_layout(int* out) { out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE; }
+// scratch offset of a named per-env array (DM_SCRATCH_PERSIST / DM_SCRATCH_UNION), or model offset of a model array (DM_ARRAYS)
+int devsim_offset(void* p, const char* name, int model_array) {
+  const DMHead* h = (const DMHead*)((DevModel*)p)->model.data();
+  if (model_array) {
+#define X(nm, w, kind) if (strcmp(name, #nm) == 0) return h->o_##nm;
+    DM_ARRAYS(X)
+#undef X
+    return -1;
+  }
+#define X(nm, words) if (strcmp(name, #nm) == 0) return h->s_##nm;
+  DM_SCRATCH_PERSIST(X)
+#undef X
+#define X(nm) if (strcmp(name, #nm) == 0) return h->s_##nm;
+  DM_SCRATCH_UNION(X)
+#undef X
+  return -1;
+}
+
+// run one stage (DEVSIM_COLLIDE, DEVSIM_KIN) of the NVP = nvp instantiation on ncase scratch images [ncase][scr_words], one block
+// each; the images are overwritten with the scratch after the stage.  Returns 0, -1 for an NVP this library does not instantiate,
+// -2 on a CUDA error.
+int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch) {
+  int rc = 0;
+  const DevModel* d = (const DevModel*)p;
+  const DMHead* h = (const DMHead*)d->model.data();
+  uint32_t* d_m = nullptr;
+  float* d_s = nullptr;
+  const size_t smem = ((size_t)h->hot_words + h->scr_words) * 4, sb = (size_t)ncase * h->scr_words * 4;
+  g_err[0] = 0;
+  DEVSIM_OK(cudaMalloc(&d_m, d->model.size() * 4));
+  DEVSIM_OK(cudaMalloc(&d_s, sb));
+  DEVSIM_OK(cudaMemcpy(d_m, d->model.data(), d->model.size() * 4, cudaMemcpyHostToDevice));
+  DEVSIM_OK(cudaMemcpy(d_s, scratch, sb, cudaMemcpyHostToDevice));
+  {
+    int matched = 0;
+#define DEVSIM_STAGE(V)                                                                                                      \
+    if (nvp == V) {                                                                                                          \
+      matched = 1;                                                                                                           \
+      DEVSIM_OK(cudaFuncSetAttribute(stage_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
+      stage_kernel<V><<<ncase, 32, smem>>>(d_m, stage, d_s);                                                                 \
+    }
+#if defined(B200_WIDE)
+    DEVSIM_STAGE(36)
+#elif defined(B200_KITCHEN)
+    DEVSIM_STAGE(31)
+#else
+    DEVSIM_STAGE(14) DEVSIM_STAGE(15) DEVSIM_STAGE(21) DEVSIM_STAGE(22) DEVSIM_STAGE(30)
+#endif
+#undef DEVSIM_STAGE
+    if (!matched) { snprintf(g_err, sizeof(g_err), "devsim_stage: NVP %d is not instantiated in this library", nvp); rc = -1; goto done; }
+  }
+  DEVSIM_OK(cudaGetLastError());
+  DEVSIM_OK(cudaDeviceSynchronize());
+  DEVSIM_OK(cudaMemcpy(scratch, d_s, sb, cudaMemcpyDeviceToHost));
+done:
+  cudaFree(d_m); cudaFree(d_s);
+  return rc;
+}
 }

@@ -89,6 +89,14 @@ def lib(wide=False):
         L.hostsim_env_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 7
         L.hostsim_spd.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
         L.hostsim_spd.restype = ctypes.c_int
+        L.hostsim_collide.argtypes = [ctypes.c_void_p, ctypes.c_int]
+        L.hostsim_collide.restype = None
+        L.hostsim_model_offset.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
+        L.hostsim_model.restype = ctypes.POINTER(ctypes.c_uint32)
+        L.hostsim_model.argtypes = [ctypes.c_void_p]
+        L.hostsim_model_words.argtypes = [ctypes.c_void_p]
+        L.hostsim_layout.argtypes = [ctypes.c_void_p]
+        L.hostsim_layout.restype = None
         assert L.hostsim_task_size() == ctypes.sizeof(FetchTaskC)
         _LIB[wide] = L
     return _LIB[wide]
@@ -151,6 +159,32 @@ class HostSim:
 
     def kinematics(self):
         self._L.hostsim_kinematics(self._h)
+
+    def collide(self, nvp):
+        """The collision stage alone, compiled as forward<nvp> compiles it (HF, CX)."""
+        self._L.hostsim_collide(self._h, int(nvp))
+
+    def offset(self, name):
+        o = self._L.hostsim_offset(self._h, name.encode())
+        assert o >= 0, name
+        return o
+
+    def model_offset(self, name):
+        o = self._L.hostsim_model_offset(self._h, name.encode())
+        assert o >= 0, name
+        return o
+
+    @property
+    def layout(self):
+        """This flavor's contact-record and group layout (dmodel.h enums)."""
+        lay = np.zeros(6, np.int32)
+        self._L.hostsim_layout(lay.ctypes.data)
+        return dict(zip(("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE"), lay.tolist()))
+
+    @property
+    def words(self):
+        """The device model buffer (header and arrays, 4-byte words)."""
+        return np.ctypeslib.as_array(self._L.hostsim_model(self._h), shape=(self._L.hostsim_model_words(self._h),))
 
     def forward(self):
         self._L.hostsim_forward(self._h)

@@ -89,6 +89,25 @@ int hostsim_offset(void* p, const char* name) {
 void hostsim_forward(void* p) { warp_call(((HostSim*)p)->ctx, [](const Ctx& c) { forward<HOST_NVP>(c, true); }); }
 void hostsim_step(void* p, int n) { warp_call(((HostSim*)p)->ctx, [n](const Ctx& c) { for (int i = 0; i < n; i++) { forward<HOST_NVP>(c, true); euler_step<HOST_NVP>(c); } }); }
 void hostsim_kinematics(void* p) { warp_call(((HostSim*)p)->ctx, [](const Ctx& c) { kinematics(c); com_quantities(c); mass_matrix(c); }); }
+// the collision stage alone, with HF and CX derived from nvp as forward<NVP> derives them (the broad phase reads the pair list of the
+// kitchen groups build through ctx.mg, the whole model)
+void hostsim_collide(void* p, int nvp) {
+  const Ctx& base = ((HostSim*)p)->ctx;
+  const bool hf = nvp >= 30, cx = nvp == 22 || nvp >= 30;
+  if (hf) warp_call(base, [](const Ctx& c) { collision<true, true>(c); });
+  else if (cx) warp_call(base, [](const Ctx& c) { collision<false, true>(c); });
+  else warp_call(base, [](const Ctx& c) { collision<false, false>(c); });
+}
+int hostsim_model_offset(void* p, const char* name) {
+  const DMHead* h = ((HostSim*)p)->ctx.h;
+#define X(nm, w, kind) if (strcmp(name, #nm) == 0) return h->o_##nm;
+  DM_ARRAYS(X)
+#undef X
+  return -1;
+}
+const uint32_t* hostsim_model(void* p) { return ((HostSim*)p)->model.data(); }
+// this flavor's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE
+void hostsim_layout(int* out) { out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE; }
 int hostsim_task_size() { return (int)sizeof(FetchTask); }
 int hostsim_env_step(void* p, const FetchTask* t, int mode, int nraw, float* st, const float* action, float* obs, float* achieved,
                      float* desired, float* reward, float* success) {
