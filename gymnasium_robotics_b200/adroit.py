@@ -22,10 +22,12 @@ from typing import Optional
 import numpy as np
 import torch
 
+from . import rotations
 from ._lib import FetchTaskC
-from .fetch import CudaBackend, FetchVectorEnv
+from .fetch import CudaBackend
 from .models import load_model
-from .spaces import Box, batch_space
+from .spaces import Box
+from .vector import VectorEnv
 
 ADROIT_REF_POINT = (0.0, -0.2, 0.2)   # fixed world point of the spatial algebra: inside the hand's workspace
 FRAME_SKIP = 5
@@ -101,88 +103,69 @@ def make_door_task(model, reward_type, frame_skip=FRAME_SKIP):
     return t
 
 
-class AdroitHammerVectorEnv(FetchVectorEnv):
-    """Observations (46), rewards and flags are float32 / bool torch tensors on `device` with a leading `num_envs` axis;
-    `info["success"]` mirrors the reference's `dict(success=goal_achieved)`."""
+class _AdroitVectorEnv(VectorEnv):
+    """Observations, rewards and flags are float32 / bool torch tensors on `device` with a leading `num_envs` axis;
+    `info["success"]` mirrors the reference's `dict(success=goal_achieved)`.  A task class names its model and task struct and
+    gives two tables:
+      * RESET_DRAWS: reset_model's uniform draws, in the reference's order: (record field, offset inside it, low, high); the
+        field "euler" is Euler angle `offset` of the orientation written to penv[3:7] (the Pen's target);
+      * STATE_KEYS: the get_env_state / set_env_state entries besides qpos and qvel: (key, record field, offset inside it, width)."""
 
     metadata = {"render_modes": [], "render_fps": 100, "autoreset_mode": "next_step"}
-    TASK_NAME, MODEL_NAME = "AdroitHandHammer", "adroit_hammer"
-    make_task = staticmethod(make_hammer_task)
-    # rng_mode="device" (b200sim_reset_uniform): (record field, offset inside it, low, high) per draw, in the reference's draw order
-    DEVICE_RESET = (("penv", 2, BOARD_Z_RANGE[0], BOARD_Z_RANGE[1]),)                                       # adroit_hammer.py:372-378
+    RECOVERY_KEEP = ("goal", "penv")   # a recovered env keeps its per-episode model pose and target
+    SUCCESS_KEY = "success"
 
     def __init__(self, num_envs: int = 1, reward_type: str = "dense", max_episode_steps: Optional[int] = 200, device="cuda:0",
                  rng_mode: str = "auto", autoreset_mode: str = "next_step", frame_skip: int = FRAME_SKIP, backend_factory=None,
                  model=None, **kwargs):
         if reward_type.lower() not in ("sparse", "dense"):
             raise ValueError(f"Unknown reward type, expected `dense` or `sparse` but got {reward_type}")   # adroit_hammer.py:224-227
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
         self.task_name, self.reward_type = self.TASK_NAME, reward_type.lower()
         self.sparse_reward = self.reward_type == "sparse"
-        self.num_envs, self.max_episode_steps, self.autoreset_mode = int(num_envs), max_episode_steps, autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
-        self.n_substeps = self.frame_skip = int(frame_skip)
-        self.model = model if model is not None else load_model(self.MODEL_NAME)
-        m = self.model
-        self.task = self.make_task(m, self.reward_type, frame_skip)
-        factory = backend_factory or _AdroitBackend
-        self.backend = factory(m, np.zeros((0, 11)), self.task, self.num_envs, device)
-        self.device = self.backend.device
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self.env_offset = int(kwargs.get("env_offset", 0))
-        self.auto_recover = bool(kwargs.get("auto_recover", False))   # opt-in NaN / huge-value scan after every step (fetch.py)
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)] \
-            if self.rng_mode == "numpy" else None
-        self._gen = torch.Generator(device=self.device)
-        self._gen.seed()
-        self._dev_seed = int(self._gen.initial_seed())
-        lay = self.backend.layout
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu),
-                                                              ("goal", 3), ("penv", 7))}
-        self.dt = float(m.opt[0] * frame_skip)
-        self.single_action_space = Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32)            # adroit_hammer.py:229-232
-        self.single_observation_space = Box(-np.inf, np.inf, shape=(int(self.task.nobs),), dtype=np.float64)
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
-        self._elapsed = self.backend.elapsed                      # library-owned step counters (in-kernel TimeLimit)
-        self.backend.set_time_limit(max_episode_steps, False)
-        self._needs_reset = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        self.frame_skip = int(frame_skip)
+        m = model if model is not None else load_model(self.MODEL_NAME)
+        t = self.make_task(m, self.reward_type, frame_skip)
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 3), ("penv", 7)),
+                         action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32),                  # adroit_hammer.py:229-232
+                         observation_space=Box(-np.inf, np.inf, shape=(int(t.nobs),), dtype=np.float64),
+                         backend_factory=backend_factory or _AdroitBackend, num_envs=num_envs, device=device,
+                         max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
+                         n_substeps=frame_skip, kwargs=kwargs)
         self.init_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)   # MujocoEnv: data.qpos at load
         self.init_qvel = torch.zeros(m.nv, dtype=torch.float32, device=self.device)
         # model pose (position 3 + quaternion 4) of the body whose pose is per-env state
-        self._board_pos0 = torch.as_tensor(np.concatenate([np.asarray(m.body_pos).reshape(-1, 3)[self.task.penv_body],
-                                                           np.asarray(m.body_quat).reshape(-1, 4)[self.task.penv_body]]),
+        self._board_pos0 = torch.as_tensor(np.concatenate([np.asarray(m.body_pos).reshape(-1, 3)[t.penv_body],
+                                                           np.asarray(m.body_quat).reshape(-1, 4)[t.penv_body]]),
                                            dtype=torch.float32, device=self.device)
         cr = np.asarray(m.act_ctrlrange, dtype=np.float64).reshape(-1, 2)
         self.act_mean, self.act_rng = cr.mean(axis=1), 0.5 * (cr[:, 1] - cr[:, 0])                      # adroit_hammer.py:271-274
-        self._last = None
-        self.closed = False
+        self._draw_bounds = tuple(torch.tensor([d[i] for d in self.RESET_DRAWS], dtype=torch.float32, device=self.device) for i in (2, 3))
 
     # ------------------------------------------------------------------ reset
+    def _rest_record(self):
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)   # ctrl, warm start, time <- 0
+        rest[self._sl["qpos"]] = self.init_qpos
+        rest[self._sl["qvel"]] = self.init_qvel
+        rest[self._sl["penv"]] = self._board_pos0
+        return rest
+
     def _device_reset(self, mask, out):
         """rng_mode="device": the uniform draws of reset_model happen inside the library (csrc/reset_sample.cuh)."""
-        if getattr(self, "_dev_reset", None) is None:
+        if self._dev_reset is None:
             from ._lib import UniformResetC
 
             p, sl = UniformResetC(), self._sl
-            p.n = len(self.DEVICE_RESET)
+            p.n = len(self.RESET_DRAWS)
             p.quat_slot = -1
-            for k, (field, off, lo, hi) in enumerate(self.DEVICE_RESET):
-                if field == "euler":      # Euler angle `off` of the orientation written to penv[3:7] (the Pen's target)
+            for k, (field, off, lo, hi) in enumerate(self.RESET_DRAWS):
+                if field == "euler":
                     p.slot[k], p.quat_slot = -1 - off, sl["penv"].start + 3
                 else:
                     p.slot[k] = sl[field].start + off
                 p.lo[k], p.hi[k] = lo, hi
-            rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)   # ctrl, warm start, time <- 0
-            rest[sl["qpos"]] = self.init_qpos
-            rest[sl["qvel"]] = self.init_qvel
-            rest[sl["penv"]] = self._board_pos0
-            self._dev_reset = (p, rest)
+            self._dev_reset = (p, self._rest)
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
-        every = getattr(self, "_reset_all", False)
+        every = self._reset_all
         p, rest = self._dev_reset
         self.backend.reset_uniform(None if every else mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)
         if every:
@@ -190,40 +173,33 @@ class AdroitHammerVectorEnv(FetchVectorEnv):
         else:
             self._elapsed.masked_fill_(mask, 0)
 
-    def _recovery_record(self):
-        """A recovered env restarts from the model's rest state and keeps its per-episode model pose and target."""
-        from ._lib import KeepC
-
-        sl, keep = self._sl, KeepC()
-        keep.n = 2
-        keep.start[0], keep.len[0] = sl["goal"].start, 3
-        keep.start[1], keep.len[1] = sl["penv"].start, 7
-        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
-        rest[sl["qpos"]] = self.init_qpos
-        rest[sl["qvel"]] = self.init_qvel
-        rest[sl["penv"]] = self._board_pos0
-        return rest, keep
-
-    def _reset_envs(self, mask, out):
-        """MujocoEnv.reset -> mj_resetData -> reset_model (adroit_hammer.py:372-378) for the envs in `mask`."""
+    def _reset_envs(self, mask, out, options=None):
+        """MujocoEnv.reset -> mj_resetData -> reset_model (the RESET_DRAWS, in the reference's order) for the envs in `mask`."""
         if self.rng_mode == "device":
             return self._device_reset(mask, out)
         idx = self._mask_indices(mask)
-        if idx.numel() == 0:
-            return
         n = idx.numel()
-        st, sl = self.backend.state, self._sl
-        lo, hi = BOARD_Z_RANGE
+        if n == 0:
+            return
         if self.rng_mode == "numpy":
-            z = torch.as_tensor([self._np_rngs[i].uniform(low=lo, high=hi) for i in idx.tolist()], dtype=torch.float32, device=self.device)
+            u = np.array([[self._np_rngs[i].uniform(low=d[2], high=d[3]) for d in self.RESET_DRAWS] for i in idx.tolist()])
         else:
-            z = lo + (hi - lo) * torch.rand(n, generator=self._gen, device=self.device)
-        rec = torch.zeros((n, st.shape[1]), dtype=torch.float32, device=self.device)   # ctrl, warm start, time <- 0
-        rec[:, sl["qpos"]] = self.init_qpos
-        rec[:, sl["qvel"]] = self.init_qvel
-        rec[:, sl["penv"]] = self._board_pos0
-        rec[:, sl["penv"].start + 2] = z
-        st[idx] = rec
+            lo, hi = self._draw_bounds
+            u = lo + (hi - lo) * torch.rand((n, lo.numel()), generator=self._gen, device=self.device)
+        u32 = torch.as_tensor(u, dtype=torch.float32, device=self.device)
+        rec = self._rest.expand(n, -1).clone()
+        for k, (field, off, _, _) in enumerate(self.RESET_DRAWS):
+            if field != "euler":
+                rec[:, self._sl[field].start + off] = u32[:, k]
+        angles = [(k, off) for k, (field, off, _, _) in enumerate(self.RESET_DRAWS) if field == "euler"]
+        if angles:            # body_quat = euler2quat([u, u, 0]), from the float64 draws of rng_mode="numpy"
+            drawn = u if self.rng_mode == "numpy" else u32.double().cpu().numpy()
+            euler = np.zeros((n, 3))
+            for k, off in angles:
+                euler[:, off] = drawn[:, k]
+            pq = self._sl["penv"].start + 3
+            rec[:, pq:pq + 4] = torch.as_tensor(rotations.euler2quat(euler), dtype=torch.float32, device=self.device)
+        self.backend.state[idx] = rec
         self._elapsed[idx] = 0
         self.backend.refresh(mask.to(torch.uint8), out)   # set_state -> mj_forward, then _get_obs
 
@@ -231,14 +207,8 @@ class AdroitHammerVectorEnv(FetchVectorEnv):
     def _obs_dict(self, out):
         return self._cast_obs(out["obs"])
 
-    def step(self, actions):
-        obs, reward, terminated, truncated, info = super().step(actions)
-        info["success"] = info.pop("is_success") > 0.5
-        info["_success"] = info.pop("_is_success")
-        if "final_info" in info:
-            fi = info["final_info"]
-            info["final_info"] = {"success": fi["is_success"] > 0.5, "_success": fi["_is_success"]}
-        return obs, reward, terminated, truncated, info
+    def _success(self, column):
+        return column > 0.5
 
     def reset(self, *, seed=None, options=None):
         """adroit_hammer.py:359-370 (and the siblings): `options={"initial_state_dict": {...}}` sets the state after the
@@ -251,191 +221,79 @@ class AdroitHammerVectorEnv(FetchVectorEnv):
     def compute_reward(self, *a, **k):
         raise NotImplementedError("Adroit environments are not GoalEnvs (no compute_reward in the reference)")
 
-    # adroit_hammer.py:380-402, batched: dicts of [N, .] tensors
+    # adroit_*.py get_env_state / set_env_state, batched: dicts of [N, .] tensors
+    def _state_keys(self):
+        return (("qpos", "qpos", 0, self.model.nq), ("qvel", "qvel", 0, self.model.nv)) + self.STATE_KEYS
+
     def get_env_state(self):
         st, sl = self.backend.state, self._sl
-        return dict(qpos=st[:, sl["qpos"]].clone(), qvel=st[:, sl["qvel"]].clone(), board_pos=st[:, sl["penv"]][:, :3].clone(),
-                    target_pos=self._last["achieved"].clone() if self._last is not None else None)
+        return {key: st[:, sl[f].start + off:sl[f].start + off + w].clone() for key, f, off, w in self._state_keys()}
 
     def set_env_state(self, state_dict):
         st, sl = self.backend.state, self._sl
-        for key, name, width in (("qpos", "qpos", self.model.nq), ("qvel", "qvel", self.model.nv), ("board_pos", "penv", 3)):
+        for key, f, off, width in self._state_keys():
             v = torch.as_tensor(np.asarray(state_dict[key]) if not torch.is_tensor(state_dict[key]) else state_dict[key])
             assert v.shape[-1] == width, f"The state dictionary entry {key} must have {width} columns"
-            st[:, sl[name].start:sl[name].start + width] = v.to(self.device, torch.float32).reshape(-1, width).expand(self.num_envs, width)
+            start = sl[f].start + off
+            st[:, start:start + width] = v.to(self.device, torch.float32).reshape(-1, width).expand(self.num_envs, width)
         st[:, sl["warm"]] = 0
         out = self.backend.new_outputs()
         self.backend.refresh(None, out)   # set_state -> mj_forward
         self._last = out
         return out["obs"]
+class AdroitHammerVectorEnv(_AdroitVectorEnv):
+    """`gym.make_vec("AdroitHandHammer-v2", num_envs=N)`: obs 46; the nail board height (model.body_pos[nail_board].z) is per-env
+    state."""
+
+    TASK_NAME, MODEL_NAME = "AdroitHandHammer", "adroit_hammer"
+    make_task = staticmethod(make_hammer_task)
+    RESET_DRAWS = (("penv", 2, BOARD_Z_RANGE[0], BOARD_Z_RANGE[1]),)                                        # adroit_hammer.py:372-378
+    STATE_KEYS = (("board_pos", "penv", 0, 3),)                                                              # adroit_hammer.py:380-402
+
+    def get_env_state(self):
+        s = super().get_env_state()
+        s["target_pos"] = self._last["achieved"].clone() if self._last is not None else None
+        return s
 
 
-class AdroitRelocateVectorEnv(AdroitHammerVectorEnv):
+class AdroitRelocateVectorEnv(_AdroitVectorEnv):
     """`gym.make_vec("AdroitHandRelocate-v2", num_envs=N)`: 36 dofs (6-dof arm + 24 hand joints + 6-dof ball) on the wide
     build; obs 39; per-episode ball start (model.body_pos[Object] x, y) and target (model.site_pos[target]) as per-env state
     (envs/adroit_hand/adroit_relocate.py:288-402)."""
 
     TASK_NAME, MODEL_NAME = "AdroitHandRelocate", "adroit_relocate"
     make_task = staticmethod(make_relocate_task)
-    DEVICE_RESET = (("penv", 0, -0.15, 0.15), ("penv", 1, -0.15, 0.3), ("goal", 0, -0.2, 0.2), ("goal", 1, -0.2, 0.2),
-                    ("goal", 2, 0.15, 0.35))                                                                   # adroit_relocate.py:354-373
+    # body_pos of "Object" (z stays the model's), then site_pos of "target" (a world site)
+    RESET_DRAWS = (("penv", 0, -0.15, 0.15), ("penv", 1, -0.15, 0.3), ("goal", 0, -0.2, 0.2), ("goal", 1, -0.2, 0.2),
+                   ("goal", 2, 0.15, 0.35))                                                                    # adroit_relocate.py:354-373
+    STATE_KEYS = (("obj_pos", "penv", 0, 3), ("target_pos", "goal", 0, 3))                                     # adroit_relocate.py:375-402
 
-    def _reset_envs(self, mask, out):
-        """reset_model (adroit_relocate.py:354-373): five uniform draws in the reference's order."""
-        if self.rng_mode == "device":
-            return self._device_reset(mask, out)
-        idx = self._mask_indices(mask)
-        if idx.numel() == 0:
-            return
-        n = idx.numel()
-        st, sl = self.backend.state, self._sl
-        lo = np.array([-0.15, -0.15, -0.2, -0.2, 0.15])
-        hi = np.array([0.15, 0.3, 0.2, 0.2, 0.35])
-        if self.rng_mode == "numpy":
-            u = torch.as_tensor(np.array([[self._np_rngs[i].uniform(low=lo[k], high=hi[k]) for k in range(5)] for i in idx.tolist()]),
-                                dtype=torch.float32, device=self.device)
-        else:
-            lo_t, hi_t = (torch.as_tensor(x, dtype=torch.float32, device=self.device) for x in (lo, hi))
-            u = lo_t + (hi_t - lo_t) * torch.rand((n, 5), generator=self._gen, device=self.device)
-        rec = torch.zeros((n, st.shape[1]), dtype=torch.float32, device=self.device)
-        rec[:, sl["qpos"]] = self.init_qpos
-        rec[:, sl["qvel"]] = self.init_qvel
-        rec[:, sl["penv"]] = self._board_pos0                       # body_pos of "Object": z stays the model's
-        rec[:, sl["penv"].start:sl["penv"].start + 2] = u[:, 0:2]
-        rec[:, sl["goal"]] = u[:, 2:5]                              # site_pos of "target" (a world site)
-        st[idx] = rec
-        self._elapsed[idx] = 0
-        self.backend.refresh(mask.to(torch.uint8), out)
-
-    # adroit_relocate.py:375-402
     def get_env_state(self):
-        st, sl = self.backend.state, self._sl
+        s = super().get_env_state()
         hand = self._last["obs"][:, -9:-6] if self._last is not None else None   # palm - ball; palm = that + ball
-        ball = self._last["achieved"] if self._last is not None else None
-        return dict(qpos=st[:, sl["qpos"]].clone(), qvel=st[:, sl["qvel"]].clone(),
-                    hand_pos=(hand + ball).clone() if hand is not None else None,
-                    obj_pos=st[:, sl["penv"]][:, :3].clone(), target_pos=st[:, sl["goal"]].clone())
-
-    def set_env_state(self, state_dict):
-        st, sl = self.backend.state, self._sl
-        for key, name, width in (("qpos", "qpos", self.model.nq), ("qvel", "qvel", self.model.nv), ("obj_pos", "penv", 3),
-                                 ("target_pos", "goal", 3)):
-            v = torch.as_tensor(np.asarray(state_dict[key]) if not torch.is_tensor(state_dict[key]) else state_dict[key])
-            assert v.shape[-1] == width, f"The state dictionary entry {key} must have {width} columns"
-            st[:, sl[name].start:sl[name].start + width] = v.to(self.device, torch.float32).reshape(-1, width).expand(self.num_envs, width)
-        st[:, sl["warm"]] = 0
-        out = self.backend.new_outputs()
-        self.backend.refresh(None, out)
-        self._last = out
-        return out["obs"]
+        s["hand_pos"] = (hand + self._last["achieved"]).clone() if hand is not None else None
+        return s
 
 
-class AdroitPenVectorEnv(AdroitHammerVectorEnv):
+class AdroitPenVectorEnv(_AdroitVectorEnv):
     """`gym.make_vec("AdroitHandPen-v2", num_envs=N)`: 30 dofs (24 hand joints + 6-dof pen; the arm is fixed), obs 45; the
     target orientation (model.body_quat[target], two Euler angles ~ U(-1, 1)) is per-env state
     (envs/adroit_hand/adroit_pen.py:288-430)."""
 
     TASK_NAME, MODEL_NAME = "AdroitHandPen", "adroit_pen"
-    DEVICE_RESET = (("euler", 0, -1.0, 1.0), ("euler", 1, -1.0, 1.0))    # adroit_pen.py:379-384: body_quat[target] = euler2quat([u, u, 0])
     make_task = staticmethod(make_pen_task)
-
-    def _reset_envs(self, mask, out):
-        """reset_model (adroit_pen.py:379-399)."""
-        if self.rng_mode == "device":
-            return self._device_reset(mask, out)
-        from . import rotations
-
-        idx = self._mask_indices(mask)
-        if idx.numel() == 0:
-            return
-        n = idx.numel()
-        st, sl = self.backend.state, self._sl
-        e = np.zeros((n, 3))
-        if self.rng_mode == "numpy":
-            for k, i in enumerate(idx.tolist()):
-                e[k, 0] = self._np_rngs[i].uniform(low=-1, high=1)
-                e[k, 1] = self._np_rngs[i].uniform(low=-1, high=1)
-        else:
-            e[:, :2] = (torch.rand((n, 2), generator=self._gen, device=self.device) * 2 - 1).double().cpu().numpy()
-        quat = torch.as_tensor(rotations.euler2quat(e), dtype=torch.float32, device=self.device)
-        rec = torch.zeros((n, st.shape[1]), dtype=torch.float32, device=self.device)
-        rec[:, sl["qpos"]] = self.init_qpos
-        rec[:, sl["qvel"]] = self.init_qvel
-        rec[:, sl["penv"]] = self._board_pos0
-        rec[:, sl["penv"].start + 3:sl["penv"].start + 7] = quat
-        st[idx] = rec
-        self._elapsed[idx] = 0
-        self.backend.refresh(mask.to(torch.uint8), out)
-
-    # adroit_pen.py:401-430
-    def get_env_state(self):
-        st, sl = self.backend.state, self._sl
-        return dict(qpos=st[:, sl["qpos"]].clone(), qvel=st[:, sl["qvel"]].clone(), desired_orien=st[:, sl["penv"]][:, 3:7].clone())
-
-    def set_env_state(self, state_dict):
-        st, sl = self.backend.state, self._sl
-        for key, start, width in (("qpos", sl["qpos"].start, self.model.nq), ("qvel", sl["qvel"].start, self.model.nv),
-                                  ("desired_orien", sl["penv"].start + 3, 4)):
-            v = torch.as_tensor(np.asarray(state_dict[key]) if not torch.is_tensor(state_dict[key]) else state_dict[key])
-            assert v.shape[-1] == width, f"The state dictionary entry {key} must have {width} columns"
-            st[:, start:start + width] = v.to(self.device, torch.float32).reshape(-1, width).expand(self.num_envs, width)
-        st[:, sl["warm"]] = 0
-        out = self.backend.new_outputs()
-        self.backend.refresh(None, out)
-        self._last = out
-        return out["obs"]
+    RESET_DRAWS = (("euler", 0, -1.0, 1.0), ("euler", 1, -1.0, 1.0))    # adroit_pen.py:379-384: body_quat[target] = euler2quat([u, u, 0])
+    STATE_KEYS = (("desired_orien", "penv", 3, 4),)                      # adroit_pen.py:401-430
 
 
-class AdroitDoorVectorEnv(AdroitHammerVectorEnv):
+class AdroitDoorVectorEnv(_AdroitVectorEnv):
     """`gym.make_vec("AdroitHandDoor-v2", num_envs=N)`: 30 dofs (4-dof arm + 24 hand joints + door hinge + latch), obs 39; the
     door frame position (model.body_pos[frame]) is per-env state (envs/adroit_hand/adroit_door.py:279-402)."""
 
     TASK_NAME, MODEL_NAME = "AdroitHandDoor", "adroit_door"
-    DEVICE_RESET = (("penv", 0, -0.3, -0.2), ("penv", 1, 0.25, 0.35), ("penv", 2, 0.252, 0.35))              # adroit_door.py:359-371
     make_task = staticmethod(make_door_task)
-
-    def _reset_envs(self, mask, out):
-        """reset_model (adroit_door.py:359-371): three uniform draws (x, y, z of the frame)."""
-        if self.rng_mode == "device":
-            return self._device_reset(mask, out)
-        idx = self._mask_indices(mask)
-        if idx.numel() == 0:
-            return
-        n = idx.numel()
-        st, sl = self.backend.state, self._sl
-        lo, hi = np.array([-0.3, 0.25, 0.252]), np.array([-0.2, 0.35, 0.35])
-        if self.rng_mode == "numpy":
-            u = torch.as_tensor(np.array([[self._np_rngs[i].uniform(low=lo[k], high=hi[k]) for k in range(3)] for i in idx.tolist()]),
-                                dtype=torch.float32, device=self.device)
-        else:
-            lo_t, hi_t = (torch.as_tensor(x, dtype=torch.float32, device=self.device) for x in (lo, hi))
-            u = lo_t + (hi_t - lo_t) * torch.rand((n, 3), generator=self._gen, device=self.device)
-        rec = torch.zeros((n, st.shape[1]), dtype=torch.float32, device=self.device)
-        rec[:, sl["qpos"]] = self.init_qpos
-        rec[:, sl["qvel"]] = self.init_qvel
-        rec[:, sl["penv"]] = self._board_pos0
-        rec[:, sl["penv"].start:sl["penv"].start + 3] = u
-        st[idx] = rec
-        self._elapsed[idx] = 0
-        self.backend.refresh(mask.to(torch.uint8), out)
-
-    # adroit_door.py:373-402
-    def get_env_state(self):
-        st, sl = self.backend.state, self._sl
-        return dict(qpos=st[:, sl["qpos"]].clone(), qvel=st[:, sl["qvel"]].clone(), door_body_pos=st[:, sl["penv"]][:, :3].clone())
-
-    def set_env_state(self, state_dict):
-        st, sl = self.backend.state, self._sl
-        for key, start, width in (("qpos", sl["qpos"].start, self.model.nq), ("qvel", sl["qvel"].start, self.model.nv),
-                                  ("door_body_pos", sl["penv"].start, 3)):
-            v = torch.as_tensor(np.asarray(state_dict[key]) if not torch.is_tensor(state_dict[key]) else state_dict[key])
-            assert v.shape[-1] == width, f"The state dictionary entry {key} must have {width} columns"
-            st[:, start:start + width] = v.to(self.device, torch.float32).reshape(-1, width).expand(self.num_envs, width)
-        st[:, sl["warm"]] = 0
-        out = self.backend.new_outputs()
-        self.backend.refresh(None, out)
-        self._last = out
-        return out["obs"]
+    RESET_DRAWS = (("penv", 0, -0.3, -0.2), ("penv", 1, 0.25, 0.35), ("penv", 2, 0.252, 0.35))               # adroit_door.py:359-371
+    STATE_KEYS = (("door_body_pos", "penv", 0, 3),)                                                           # adroit_door.py:373-402
 
 
 ADROIT_TASKS = {"AdroitHandHammer": AdroitHammerVectorEnv, "AdroitHandRelocate": AdroitRelocateVectorEnv,

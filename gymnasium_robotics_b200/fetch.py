@@ -20,8 +20,8 @@ import torch
 from . import _lib
 from .mjcf import EQ_WELD, JNT_FREE
 from .models import load_model
-from .rollout import CtorPickle
-from .spaces import Box, Dict as DictSpace, batch_space
+from .spaces import Box, Dict as DictSpace
+from .vector import VectorEnv
 
 FETCH_TASKS = {
     "FetchReach": dict(model="fetch_reach", has_object=False, block_gripper=True, gripper_extra_height=0.2,
@@ -230,11 +230,9 @@ class CudaBackend:
         return int(self.L.b200sim_launch_count(self.h))
 
 
-class FetchVectorEnv(CtorPickle):
+class FetchVectorEnv(VectorEnv):
     """`gym.make_vec("FetchPickAndPlace-v4", num_envs=N)` replacement.  Observations, rewards and flags are torch
     tensors on `device` (float32 / bool) with a leading `num_envs` axis."""
-
-    metadata = {"render_modes": [], "render_fps": 25, "autoreset_mode": "next_step"}
 
     def __init__(self, task: str = "FetchPickAndPlace", num_envs: int = 1, reward_type: str = "sparse",
                  max_episode_steps: Optional[int] = 50, device="cuda:0", rng_mode: str = "auto",
@@ -243,54 +241,20 @@ class FetchVectorEnv(CtorPickle):
             raise KeyError(f"unknown Fetch task {task!r}")
         if reward_type not in ("sparse", "dense"):
             raise ValueError("reward_type must be 'sparse' or 'dense'")
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
         cfg = dict(FETCH_TASKS[task])
         self.task_name, self.cfg, self.reward_type = task, cfg, reward_type
-        self.num_envs, self.max_episode_steps, self.autoreset_mode = int(num_envs), max_episode_steps, autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
-        self.n_substeps = n_substeps
-        self.model = load_model(cfg["model"])
-        self.task = make_task_struct(self.model, cfg, reward_type, n_substeps)
-        eq = welded_eq_data(self.model)
-        factory = backend_factory or CudaBackend
-        self.backend = factory(self.model, eq, self.task, self.num_envs, device)
-        self.device = self.backend.device
-        # "numpy": per-env PCG64 streams in the reference's draw order (value-equal resets); "torch": torch's device generator;
-        # "device": the draws happen inside the library (b200sim_reset, csrc/reset_sample.cuh) -- no host work per reset
-        if rng_mode not in ("auto", "numpy", "torch", "device"):
-            raise ValueError("rng_mode must be auto, numpy, torch or device")
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self.env_offset = int(kwargs.get("env_offset", 0))   # global index of env 0 (sharded runs, sharding.py)
-        # opt-in failure detection: after every step the state records are scanned for NaN / huge values and such envs are put
-        # back to their rest state with the goal kept ([ext] mj_checkPos / mj_checkVel / mj_checkAcc + mj_resetData inside mj_step)
-        self.auto_recover = bool(kwargs.get("auto_recover", False))
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)] \
-            if self.rng_mode == "numpy" else None
-        self._gen = torch.Generator(device=self.device)
-        self._gen.seed()
-        self._dev_seed = int(self._gen.initial_seed())
-        lay = self.backend.layout
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", self.model.nq), ("qvel", self.model.nv), ("warm", self.model.nv),
-                                                              ("ctrl", self.model.nu), ("mocap", 7), ("pose", 7), ("goal", 3))}
-        self.dt = float(self.model.opt[0] * n_substeps)
-        nobs = self.task.nobs
-        self.single_action_space = Box(-1.0, 1.0, shape=(4,), dtype=np.float32)
-        self.single_observation_space = DictSpace(dict(
-            desired_goal=Box(-np.inf, np.inf, shape=(3,), dtype=np.float64),
-            achieved_goal=Box(-np.inf, np.inf, shape=(3,), dtype=np.float64),
-            observation=Box(-np.inf, np.inf, shape=(nobs,), dtype=np.float64)))
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
-        # TimeLimit and the terminated / truncated flags are computed by the step kernel (b200sim_set_time_limit); the per-env
-        # step counters live in the library and are visible here as a tensor
-        self._elapsed = self.backend.elapsed
-        self.backend.set_time_limit(max_episode_steps, False)   # robot_env.py:106-112: compute_terminated is constant False
-        self._needs_reset = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        m = load_model(cfg["model"])
+        t = make_task_struct(m, cfg, reward_type, n_substeps)
+        box = lambda n: Box(-np.inf, np.inf, shape=(n,), dtype=np.float64)
+        # robot_env.py:106-112: compute_terminated is constant False, so the kernel's TimeLimit is the only episode end
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("mocap", 7),
+                                                  ("pose", 7), ("goal", 3)),
+                         action_space=Box(-1.0, 1.0, shape=(4,), dtype=np.float32),
+                         observation_space=DictSpace(dict(desired_goal=box(3), achieved_goal=box(3), observation=box(t.nobs))),
+                         backend_factory=backend_factory or CudaBackend, eq_data=welded_eq_data(m), num_envs=num_envs, device=device,
+                         max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
+                         n_substeps=n_substeps, kwargs=kwargs)
         self._env_setup()
-        self.closed = False
 
     # ------------------------------------------------------------------ construction
     def _env_setup(self):
@@ -319,6 +283,13 @@ class FetchVectorEnv(CtorPickle):
         self._mocap_rest = torch.tensor([0, 0, 0, 1, 0, 0, 0], dtype=torch.float32, device=self.device)
         self._obj_qadr = int(m.jnt_qposadr[m.joint_id("object0:joint")]) if self.cfg["has_object"] else -1
         self._last = out
+
+    def _rest_record(self):
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
+        rest[self._sl["qpos"]] = self.initial_qpos
+        rest[self._sl["qvel"]] = self.initial_qvel
+        rest[self._sl["mocap"]] = self._mocap_rest
+        return rest
 
     # ------------------------------------------------------------------ sampling
     def _sample_reset(self, idx):
@@ -369,14 +340,6 @@ class FetchVectorEnv(CtorPickle):
                 goals[:, 2] += torch.where(air, u(n) * 0.45, torch.zeros(n, device=self.device))
         return obj, goals
 
-    def _mask_indices(self, mask):
-        """Indices of the envs in `mask`; no device round trip when the caller knows that every env is due (`_reset_all`)."""
-        if getattr(self, "_reset_all", False):
-            if getattr(self, "_all_idx", None) is None or self._all_idx.numel() != self.num_envs:
-                self._all_idx = torch.arange(self.num_envs, device=self.device)
-            return self._all_idx
-        return torch.nonzero(mask, as_tuple=False).flatten()
-
     def _device_reset_params(self):
         from ._lib import FetchResetC
 
@@ -388,39 +351,15 @@ class FetchVectorEnv(CtorPickle):
             p.target_offset[k] = float(np.broadcast_to(np.asarray(cfg["target_offset"], dtype=np.float64), (3,))[k])
             p.gripper_xpos[k] = float(g0[k])
         p.height_offset = float(self.height_offset or 0.0)
-        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)   # mj_resetData
-        rest[self._sl["qpos"]] = self.initial_qpos
-        rest[self._sl["qvel"]] = self.initial_qvel
-        rest[self._sl["mocap"]] = self._mocap_rest
-        return p, rest
+        return p, self._rest
 
-    def _recovery_record(self):
-        """(rest record, ranges of the state record a recovered env keeps) for b200sim_check_state."""
-        from ._lib import KeepC
-
-        keep = KeepC()
-        keep.n, keep.start[0], keep.len[0] = 1, self._sl["goal"].start, self._sl["goal"].stop - self._sl["goal"].start
-        return self._device_reset_params()[1], keep
-
-    def _check_and_recover(self, out, info):
-        if getattr(self, "_recovery", None) is None:
-            self._recovery = self._recovery_record()
-            self._bad = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
-            self.bad_state_count = torch.zeros((), dtype=torch.int64, device=self.device)
-        rest, keep = self._recovery
-        self.backend.check_state(self._bad, rest, keep)
-        self.backend.refresh(self._bad, out)          # mj_forward + _get_obs of the recovered envs (none, almost always)
-        bad = self._bad.bool()
-        self.bad_state_count += bad.sum()
-        info["bad_state"] = bad
-
-    def _reset_envs(self, mask, out):
+    def _reset_envs(self, mask, out, options=None):
         if self.rng_mode == "device":
-            if getattr(self, "_dev_reset", None) is None:
+            if self._dev_reset is None:
                 self._dev_reset = self._device_reset_params()
                 self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
-            every = getattr(self, "_reset_all", False)
             p, rest = self._dev_reset
+            every = self._reset_all
             self.backend.reset_draw(None if every else mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)
             if every:
                 self._elapsed.zero_()
@@ -432,146 +371,10 @@ class FetchVectorEnv(CtorPickle):
             return
         st, sl = self.backend.state, self._sl
         obj, goals = self._sample_reset(idx)
-        rec = torch.zeros((idx.numel(), st.shape[1]), dtype=torch.float32, device=self.device)  # mj_resetData
-        rec[:, sl["qpos"]] = self.initial_qpos
-        rec[:, sl["qvel"]] = self.initial_qvel
-        rec[:, sl["mocap"]] = self._mocap_rest
+        rec = self._rest.expand(idx.numel(), -1).clone()  # mj_resetData
         if obj is not None:
-            rec[:, self._sl["qpos"].start + self._obj_qadr: self._sl["qpos"].start + self._obj_qadr + 2] = obj
+            rec[:, sl["qpos"].start + self._obj_qadr: sl["qpos"].start + self._obj_qadr + 2] = obj
         rec[:, sl["goal"]] = goals
         st[idx] = rec
         self._elapsed[idx] = 0
         self.backend.refresh(mask.to(torch.uint8), out)  # mj_forward + _get_obs for the reset envs
-
-    # ------------------------------------------------------------------ gymnasium API
-    def _obs_dict(self, out):
-        return self._cast_obs({"observation": out["obs"], "achieved_goal": out["achieved"], "desired_goal": out["desired"]})
-
-    def reset(self, *, seed=None, options=None):
-        if seed is not None:
-            seeds = [seed + i for i in range(self.num_envs)] if isinstance(seed, (int, np.integer)) else list(seed)
-            if self.rng_mode == "numpy":
-                self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(s))) for s in seeds]
-            self._gen.manual_seed(int(seeds[0]))
-            if self.rng_mode == "device":   # one key for the batch; env index and episode counter select the stream
-                self._dev_seed = int(seeds[0])
-                if getattr(self, "_episode", None) is not None:
-                    self._episode.zero_()
-        out = self.backend.new_outputs()
-        mask = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
-        self._reset_all = True
-        try:
-            self._reset_envs(mask, out)
-        finally:
-            self._reset_all = False
-        self._needs_reset.zero_()
-        self._elapsed_ub, self._pending_reset = 0, False
-        self._in_phase = True   # every env has the same step count (these envs never terminate): TimeLimit is host-known
-        self._last = out
-        return self._obs_dict(out), {}
-
-    def step(self, actions):
-        if not torch.is_tensor(actions):
-            actions = torch.as_tensor(np.asarray(actions, dtype=np.float32))
-        if tuple(actions.shape) != (self.num_envs, self.single_action_space.shape[0]):
-            raise ValueError("Action dimension mismatch")
-        actions = actions.to(self.device, torch.float32, non_blocking=True).contiguous()
-        out = self.backend.new_outputs()
-        # clip + _set_action + n_substeps x mj_step + _get_obs + reward + TimeLimit / terminated / truncated: one kernel
-        self.backend.step(actions, out)
-        self._elapsed_ub = getattr(self, "_elapsed_ub", 0) + 1   # host-side upper bound of max(_elapsed): no sync on most steps
-        reward, success = out["reward"], out["success"]
-        terminated, truncated = out["terminated"], out["truncated"]
-        # solver_info: Newton iterations (low 16 bits) | capacity-overflow flags << 16 of this step, per env (the backend's
-        # persistent tensor: valid until the next step); solver_overflow_count: device counter over the env's lifetime
-        info = {"is_success": success, "solver_info": self.backend.info}
-        if getattr(self, "auto_recover", False):
-            self._check_and_recover(out, info)
-        if getattr(self, "_const_true", None) is None or self._const_true.numel() != self.num_envs:
-            self._const_true = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
-        in_phase = getattr(self, "_in_phase", False)
-        if self.autoreset_mode == "next_step" and getattr(self, "_pending_reset", False):
-            self._pending_reset = False
-            if in_phase or bool(self._needs_reset.any()):
-                self._reset_all = in_phase
-                # envs that finished on the previous call are reset now; their action is ignored (gymnasium NEXT_STEP)
-                pre = self._needs_reset.clone()
-                self._reset_envs(pre, out)
-                self._mask_step_outputs(out, pre)
-                self._needs_reset.zero_()
-                self._reset_all = False
-                self._elapsed_ub = 0 if in_phase else int(self._elapsed.max())
-        # TimeLimit: the flags come from the kernel; the host only looks at them (and synchronises) once the bound says an env may be due
-        may_truncate = self.max_episode_steps is not None and self._elapsed_ub >= self.max_episode_steps
-        if may_truncate:
-            done = truncated | terminated
-            if self.autoreset_mode == "next_step":
-                self._needs_reset = done
-                self._pending_reset = True
-            elif self.autoreset_mode == "same_step":
-                # in phase (all envs reset together and none terminates): the bound IS every env's step count -- no device read
-                if in_phase or bool(done.any()):
-                    fo = self._obs_dict(out)
-                    info["final_obs"] = {k: v.clone() for k, v in fo.items()} if isinstance(fo, dict) else fo.clone()
-                    info["_final_obs"] = done.clone()
-                    # gymnasium's SAME_STEP convention: the info of the finished episodes next to their last observation
-                    info["final_info"] = {"is_success": success.clone(), "_is_success": done.clone()}
-                    info["_final_info"] = done.clone()
-                    self._reset_all = in_phase
-                    self._reset_envs(done, out)
-                    self._reset_all = False
-                self._elapsed_ub = 0 if in_phase else int(self._elapsed.max())
-        info["_is_success"] = self._const_true
-        self._last = out
-        return self._obs_dict(out), reward, terminated, truncated, info
-
-    def _mask_step_outputs(self, out, pre):
-        """NEXT_STEP autoreset: the envs in `pre` were reset instead of stepped -- reward 0, no success, no flags (in place, so the
-        packed row stays the single source of the step's results)."""
-        k = self.backend.nobs + 2 * self.backend.ngoal
-        out["packed"][:, k:k + 4].masked_fill_(pre[:, None], 0.0)
-        out["flags"].masked_fill_(pre[None, :], 0)
-
-    @property
-    def solver_overflow_count(self):
-        """Env-steps so far in which a capacity limit (broad-phase candidates, contacts, contact groups, limit rows) dropped
-        something (DESIGN.md deviation 5); reads the device counter (synchronises)."""
-        return int(self.backend.overflow_counter[0])
-
-    # GoalEnv API (core.py:45-114), batched; accepts numpy or torch, any leading shape
-    def compute_reward(self, achieved_goal, desired_goal, info=None):
-        is_np = not torch.is_tensor(achieved_goal)
-        ag = torch.as_tensor(np.asarray(achieved_goal)) if is_np else achieved_goal
-        dg = torch.as_tensor(np.asarray(desired_goal)) if not torch.is_tensor(desired_goal) else desired_goal
-        lead = ag.shape[:-1]
-        r = self.backend.compute_reward(ag, dg).reshape(lead)
-        if is_np:
-            r = r.cpu().numpy()
-            return r.astype(np.float32) if self.reward_type == "sparse" else r.astype(np.float64)
-        return r
-
-    def compute_terminated(self, achieved_goal, desired_goal, info=None):
-        return False
-
-    def compute_truncated(self, achieved_goal, desired_goal, info=None):
-        return False
-
-    # state access (checkpoint / parity injection), SURVEY.md section 5
-    def get_state(self):
-        return self.backend.state.clone(), self._elapsed.clone()
-
-    def set_state(self, state, elapsed=None):
-        self.backend.state.copy_(state)
-        if elapsed is not None:
-            self._elapsed.copy_(elapsed)
-            self._in_phase = False
-        self._elapsed_ub = int(self._elapsed.max())
-        out = self.backend.new_outputs()
-        self.backend.refresh(None, out)
-        self._last = out
-        return self._obs_dict(out)
-
-    def close(self):
-        if not getattr(self, "closed", True):
-            self.backend.close()
-            self.closed = True

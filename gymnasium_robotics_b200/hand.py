@@ -20,9 +20,10 @@ import torch
 
 from . import rotations
 from ._lib import FetchTaskC
-from .fetch import CudaBackend, FetchVectorEnv, N_SUBSTEPS
+from .fetch import CudaBackend, N_SUBSTEPS
 from .models import load_model
-from .spaces import Box, Dict as DictSpace, batch_space
+from .spaces import Box, Dict as DictSpace
+from .vector import VectorEnv
 
 # target_position / target_rotation of the registered ids (__init__.py:105-395); TARGET_POSITION_RANGE manipulate_block.py:226
 HAND_TASKS = {
@@ -76,10 +77,13 @@ class _HandBackend(CudaBackend):
     REF = HAND_REF_POINT
 
 
-class HandVectorEnv(FetchVectorEnv):
-    """Observations, rewards and flags are float32 / bool torch tensors on `device` with a leading `num_envs` axis."""
+def _goal_space(ngoal, nobs):
+    box = lambda n: Box(-np.inf, np.inf, shape=(n,), dtype=np.float64)
+    return DictSpace(dict(desired_goal=box(ngoal), achieved_goal=box(ngoal), observation=box(nobs)))
 
-    metadata = {"render_modes": [], "render_fps": 25, "autoreset_mode": "next_step"}
+
+class HandVectorEnv(VectorEnv):
+    """Observations, rewards and flags are float32 / bool torch tensors on `device` with a leading `num_envs` axis."""
 
     def __init__(self, task: str = "HandManipulateBlockRotateXYZ", num_envs: int = 1, reward_type: str = "sparse",
                  max_episode_steps: Optional[int] = 100, device="cuda:0", rng_mode: str = "auto", autoreset_mode: str = "next_step",
@@ -91,10 +95,6 @@ class HandVectorEnv(FetchVectorEnv):
             raise KeyError(f"unknown Hand task {task!r}")
         if reward_type not in ("sparse", "dense"):
             raise ValueError("reward_type must be 'sparse' or 'dense'")
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
         if relative_control:
             # hand_env.py:47-57 calls data.get_joint_qpos, which the new mujoco bindings lack: dead code for the -v1 ids
             raise NotImplementedError("relative_control is not available in the reference's -v1 envs either")
@@ -111,44 +111,21 @@ class HandVectorEnv(FetchVectorEnv):
         self.randomize_initial_position, self.randomize_initial_rotation = randomize_initial_position, randomize_initial_rotation
         self.distance_threshold, self.rotation_threshold = distance_threshold, rotation_threshold
         self.task_name, self.cfg, self.reward_type = task, cfg, reward_type
-        self.num_envs, self.max_episode_steps, self.autoreset_mode = int(num_envs), max_episode_steps, autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
-        self.n_substeps = n_substeps
         # touch_get_obs is None for the plain ids; the *TouchSensors ids pass "boolean" / "sensordata" (or "log" / "off"):
         # they use the model with the 92 touch sites (manipulate_block_touch_sensors.py:72-92)
         self.touch_get_obs = touch_get_obs
-        self.model = model if model is not None else load_model(
+        m = model if model is not None else load_model(
             cfg.get("model", "hand_block") if touch_get_obs is None else cfg.get("touch_model", "hand_block_touch"))
-        m = self.model
-        self.task = make_hand_task(m, self.target_position, self.target_rotation, reward_type, distance_threshold,
-                                   rotation_threshold, n_substeps, touch_get_obs, ignore_z_target_rotation)
-        factory = backend_factory or _HandBackend
-        self.backend = factory(m, np.zeros((0, 11)), self.task, self.num_envs, device)
-        self.device = self.backend.device
+        t = make_hand_task(m, self.target_position, self.target_rotation, reward_type, distance_threshold,
+                           rotation_threshold, n_substeps, touch_get_obs, ignore_z_target_rotation)
         # "device": start pose and goal are drawn inside the library (b200sim_reset_hand_pose / _goal, csrc/reset_sample.cuh)
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self.env_offset = int(kwargs.get("env_offset", 0))
-        self.auto_recover = bool(kwargs.get("auto_recover", False))   # opt-in NaN / huge-value scan after every step (fetch.py)
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)] \
-            if self.rng_mode == "numpy" else None
-        self._gen = torch.Generator(device=self.device)
-        self._gen.seed()
-        self._dev_seed = int(self._gen.initial_seed())
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 7)),
+                         action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32), observation_space=_goal_space(7, t.nobs),
+                         backend_factory=backend_factory or _HandBackend, num_envs=num_envs, device=device,
+                         max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
+                         n_substeps=n_substeps, kwargs=kwargs)
         lay = self.backend.layout
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 7))}
-        self._obj = slice(lay["qpos"] + self.task.obj_qadr, lay["qpos"] + self.task.obj_qadr + 7)
-        self.dt = float(m.opt[0] * n_substeps)
-        nobs = self.task.nobs
-        self.single_action_space = Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32)
-        self.single_observation_space = DictSpace(dict(
-            desired_goal=Box(-np.inf, np.inf, shape=(7,), dtype=np.float64),
-            achieved_goal=Box(-np.inf, np.inf, shape=(7,), dtype=np.float64),
-            observation=Box(-np.inf, np.inf, shape=(nobs,), dtype=np.float64)))
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
-        self._elapsed = self.backend.elapsed                      # library-owned step counters (in-kernel TimeLimit)
-        self.backend.set_time_limit(max_episode_steps, False)
-        self._needs_reset = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        self._obj = slice(lay["qpos"] + t.obj_qadr, lay["qpos"] + t.obj_qadr + 7)
         # robot_env.py:301-303 after _env_setup with initial_qpos = {} (manipulate.py:148-151)
         self.initial_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)
         self.initial_qvel = torch.zeros(m.nv, dtype=torch.float32, device=self.device)
@@ -158,8 +135,13 @@ class HandVectorEnv(FetchVectorEnv):
         self._parallel = torch.as_tensor(np.array(self._parallel_np), dtype=torch.float32, device=self.device)
         self._range = torch.as_tensor(TARGET_POSITION_RANGE, dtype=torch.float32, device=self.device)
         self.reset_attempts = 0   # total settle passes run by resets (>= number of resets; diagnostics)
-        self._last = None
-        self.closed = False
+
+    def _rest_record(self):
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
+        rest[self._sl["qpos"]] = self.initial_qpos
+        rest[self._sl["qvel"]] = self.initial_qvel
+        rest[self._sl["ctrl"]] = self._ctrl_center          # _set_action(np.zeros(20))
+        return rest
 
     # ------------------------------------------------------------------ sampling
     @staticmethod
@@ -258,21 +240,9 @@ class HandVectorEnv(FetchVectorEnv):
             quat = obj[:, 3:].clone()
         return torch.cat([pos, quat / torch.linalg.norm(quat, dim=1, keepdim=True)], dim=1)
 
-    def _recovery_record(self):
-        from ._lib import KeepC
-
-        sl, keep = self._sl, KeepC()
-        keep.n, keep.start[0], keep.len[0] = 1, sl["goal"].start, sl["goal"].stop - sl["goal"].start
-        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
-        rest[sl["qpos"]] = self.initial_qpos
-        rest[sl["qvel"]] = self.initial_qvel
-        if hasattr(self, "_ctrl_center"):
-            rest[sl["ctrl"]] = self._ctrl_center
-        return rest, keep
-
     def _device_reset(self, mask, out):
         """rng_mode="device": the same retry loop with the draws inside the library; the host only reads `pending.any()`."""
-        if getattr(self, "_dev_reset", None) is None:
+        if self._dev_reset is None:
             from ._lib import HandResetC
 
             modes = {"ignore": 0, "fixed": 0, "z": 1, "parallel": 2, "xyz": 3}
@@ -284,12 +254,7 @@ class HandVectorEnv(FetchVectorEnv):
             p.goal_rot_mode, p.goal_random_position = modes[self.target_rotation], int(self.target_position == "random")
             for k in range(3):
                 p.pos_lo[k], p.pos_hi[k] = float(TARGET_POSITION_RANGE[k, 0]), float(TARGET_POSITION_RANGE[k, 1])
-            sl = self._sl
-            rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
-            rest[sl["qpos"]] = self.initial_qpos
-            rest[sl["qvel"]] = self.initial_qvel
-            rest[sl["ctrl"]] = self._ctrl_center
-            self._dev_reset = (p, rest, self._parallel.contiguous())
+            self._dev_reset = (p, self._rest, self._parallel.contiguous())
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         p, rest, par = self._dev_reset
         st = self.backend.state
@@ -307,7 +272,7 @@ class HandVectorEnv(FetchVectorEnv):
         self.backend.reset_hand_goal(mask.to(torch.uint8), p, par, self._dev_seed, self.env_offset, self._episode, out)
         self._elapsed.masked_fill_(mask, 0)
 
-    def _reset_envs(self, mask, out):
+    def _reset_envs(self, mask, out, options=None):
         """BaseRobotEnv.reset (robot_env.py:154-186): retry `_reset_sim` until the block rests on the palm, then sample
         the goal.  Every attempt settles the pending envs together with one masked raw-step launch (10 x 20 sub-steps)."""
         if self.rng_mode == "device":
@@ -321,11 +286,8 @@ class HandVectorEnv(FetchVectorEnv):
             idx = torch.nonzero(pending, as_tuple=False).flatten()
             if idx.numel() == 0:
                 break
-            rec = torch.zeros((idx.numel(), st.shape[1]), dtype=torch.float32, device=self.device)  # time, qpos, qvel reset
-            rec[:, sl["qpos"]] = self.initial_qpos
-            rec[:, sl["qvel"]] = self.initial_qvel
+            rec = self._rest.expand(idx.numel(), -1).clone()  # time, qpos, qvel reset; _set_action(np.zeros(20))
             rec[:, self._obj] = self._sample_initial_pose(idx)
-            rec[:, sl["ctrl"]] = self._ctrl_center          # _set_action(np.zeros(20))
             rec[:, sl["goal"]] = st[idx][:, sl["goal"]]
             st[idx] = rec
             self.backend.raw_step(10 * self.n_substeps, out, mask=pending.to(torch.uint8))
@@ -337,8 +299,6 @@ class HandVectorEnv(FetchVectorEnv):
         st[idx_all, sl["goal"]] = self._sample_goals(idx_all, st[idx_all][:, self._obj])
         self._elapsed[idx_all] = 0
         self.backend.refresh(mask.to(torch.uint8), out)  # mj_forward + _get_obs for the reset envs
-
-
 
 
 # ---------------------------------------------------------------------------------------------------------------- HandReach
@@ -383,28 +343,18 @@ def body_xpos(model, qpos, body_name):
     return pos
 
 
-class HandReachVectorEnv(FetchVectorEnv):
+class HandReachVectorEnv(VectorEnv):
     """`gym.make_vec("HandReach-v3", num_envs=N)` replacement (envs/shadow_dexterous_hand/reach.py, MujocoHandReachEnv)."""
-
-    metadata = {"render_modes": [], "render_fps": 25, "autoreset_mode": "next_step"}
 
     def __init__(self, num_envs: int = 1, reward_type: str = "sparse", max_episode_steps: Optional[int] = 50, device="cuda:0",
                  rng_mode: str = "auto", autoreset_mode: str = "next_step", n_substeps: int = N_SUBSTEPS, backend_factory=None,
                  distance_threshold=0.01, relative_control=False, initial_qpos=None, model=None, **kwargs):
         if reward_type not in ("sparse", "dense"):
             raise ValueError("reward_type must be 'sparse' or 'dense'")
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
         if relative_control:
             raise NotImplementedError("relative_control is not available in the reference's new-binding envs either")
         self.task_name, self.reward_type, self.distance_threshold = "HandReach", reward_type, distance_threshold
-        self.num_envs, self.max_episode_steps, self.autoreset_mode = int(num_envs), max_episode_steps, autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
-        self.n_substeps = n_substeps
-        self.model = model if model is not None else load_model("hand_reach")
-        m = self.model
+        m = model if model is not None else load_model("hand_reach")
         t = FetchTaskC()
         t.kind, t.nact, t.ngoal = 3, int(m.nu), 15
         t.n_substeps, t.reward_dense = int(n_substeps), int(reward_type == "dense")
@@ -412,31 +362,11 @@ class HandReachVectorEnv(FetchVectorEnv):
         t.distance_threshold, t.dt = float(distance_threshold), float(m.opt[0] * n_substeps)
         for k, name in enumerate(FINGERTIP_SITE_NAMES):
             t.tip_site[k] = m.site_id(name)
-        self.task = t
-        factory = backend_factory or _HandBackend
-        self.backend = factory(m, np.zeros((0, 11)), t, self.num_envs, device)
-        self.device = self.backend.device
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self.env_offset = int(kwargs.get("env_offset", 0))
-        self.auto_recover = bool(kwargs.get("auto_recover", False))   # opt-in NaN / huge-value scan after every step (fetch.py)
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)] \
-            if self.rng_mode == "numpy" else None
-        self._gen = torch.Generator(device=self.device)
-        self._gen.seed()
-        self._dev_seed = int(self._gen.initial_seed())
-        lay = self.backend.layout
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 15))}
-        self.dt = float(m.opt[0] * n_substeps)
-        self.single_action_space = Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32)
-        self.single_observation_space = DictSpace(dict(
-            desired_goal=Box(-np.inf, np.inf, shape=(15,), dtype=np.float64),
-            achieved_goal=Box(-np.inf, np.inf, shape=(15,), dtype=np.float64),
-            observation=Box(-np.inf, np.inf, shape=(t.nobs,), dtype=np.float64)))
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
-        self._elapsed = self.backend.elapsed                      # library-owned step counters (in-kernel TimeLimit)
-        self.backend.set_time_limit(max_episode_steps, False)
-        self._needs_reset = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 15)),
+                         action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32), observation_space=_goal_space(15, t.nobs),
+                         backend_factory=backend_factory or _HandBackend, num_envs=num_envs, device=device,
+                         max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
+                         n_substeps=n_substeps, kwargs=kwargs)
         # _env_setup (reach.py:286-296): initial joint angles, mj_forward, initial fingertip positions and palm position
         q0 = np.array(m.qpos0, dtype=np.float64)
         for name, value in (initial_qpos or REACH_INITIAL_QPOS).items():
@@ -451,7 +381,12 @@ class HandReachVectorEnv(FetchVectorEnv):
         self.initial_goal = out["achieved"][0].clone()
         self.palm_xpos = body_xpos(m, q0, "robot0:palm")
         self._last = out
-        self.closed = False
+
+    def _rest_record(self):   # mj_resetData (robot_env.py:305-316)
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
+        rest[self._sl["qpos"]] = self.initial_qpos
+        rest[self._sl["qvel"]] = self.initial_qvel
+        return rest
 
     def _sample_goals(self, idx):
         """reach.py:95-121."""
@@ -487,10 +422,8 @@ class HandReachVectorEnv(FetchVectorEnv):
         goal[keep] = init_t
         return goal.reshape(n, 15)
 
-    _recovery_record = HandVectorEnv._recovery_record
-
     def _device_reset(self, mask, out):
-        if getattr(self, "_dev_reset", None) is None:
+        if self._dev_reset is None:
             from ._lib import ReachResetC
 
             p = ReachResetC()
@@ -500,27 +433,21 @@ class HandReachVectorEnv(FetchVectorEnv):
                 p.meeting[k] = float(meeting[k])
             for k in range(15):
                 p.initial_goal[k] = float(init[k])
-            rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
-            rest[self._sl["qpos"]] = self.initial_qpos
-            rest[self._sl["qvel"]] = self.initial_qvel
-            self._dev_reset = (p, rest)
+            self._dev_reset = (p, self._rest)
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         p, rest = self._dev_reset
         self.backend.reset_reach(mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)
         self._elapsed.masked_fill_(mask, 0)
 
-    def _reset_envs(self, mask, out):
+    def _reset_envs(self, mask, out, options=None):
         if self.rng_mode == "device":
             return self._device_reset(mask, out)
         idx = torch.nonzero(mask, as_tuple=False).flatten()
         if idx.numel() == 0:
             return
-        st, sl = self.backend.state, self._sl
-        rec = torch.zeros((idx.numel(), st.shape[1]), dtype=torch.float32, device=self.device)  # mj_resetData (robot_env.py:305-316)
-        rec[:, sl["qpos"]] = self.initial_qpos
-        rec[:, sl["qvel"]] = self.initial_qvel
-        rec[:, sl["goal"]] = self._sample_goals(idx)
-        st[idx] = rec
+        rec = self._rest.expand(idx.numel(), -1).clone()
+        rec[:, self._sl["goal"]] = self._sample_goals(idx)
+        self.backend.state[idx] = rec
         self._elapsed[idx] = 0
         self.backend.refresh(mask.to(torch.uint8), out)  # mj_forward + _get_obs
 

@@ -22,8 +22,8 @@ import torch
 from ._lib import FetchTaskC
 from .fetch import CudaBackend
 from .models import load_franka_config, load_model
-from .rollout import CtorPickle
-from .spaces import Box, batch_space
+from .spaces import Box
+from .vector import VectorEnv
 
 KITCHEN_REF_POINT = (-0.2, 0.3, 1.8)   # fixed world point of the spatial algebra: inside the robot's workspace
 FRAME_SKIP = 40
@@ -59,21 +59,19 @@ class _KitchenBackend(CudaBackend):
     REF = KITCHEN_REF_POINT
 
 
-class KitchenVectorEnv(CtorPickle):
+class KitchenVectorEnv(VectorEnv):
     """`gym.make_vec("FrankaKitchen-v1", num_envs=N)`.  Observation dict: `observation` [N, 59], `achieved_goal` /
     `desired_goal` dicts task -> [N, k]; reward = number of tasks completed in the step; `terminated` when every task of the
-    episode is completed; info carries the bookkeeping as boolean [N, n_tasks] tensors (column order `self.tasks`)."""
+    episode is completed; info carries the bookkeeping as boolean [N, n_tasks] tensors (column order `self.tasks`).
+    The observation is noisy, and the next step's control targets start from it, so there is no `set_state`."""
 
     metadata = {"render_modes": [], "render_fps": 12, "autoreset_mode": "next_step"}
+    AUTO_RECOVER = DEVICE_RESET = False
 
     def __init__(self, num_envs: int = 1, tasks_to_complete=None, terminate_on_tasks_completed: bool = True,
                  remove_task_when_completed: bool = True, object_noise_ratio: float = 0.0005, robot_noise_ratio: float = 0.01,
                  max_episode_steps: Optional[int] = 280, device="cuda:0", rng_mode: str = "auto", autoreset_mode: str = "next_step",
                  frame_skip: int = FRAME_SKIP, backend_factory=None, model=None, **kwargs):
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
         tasks = list(OBS_ELEMENT_GOALS.keys()) if tasks_to_complete is None else list(tasks_to_complete)
         for task in tasks:                                                      # kitchen_env.py:291-297
             if task not in OBS_ELEMENT_GOALS:
@@ -81,18 +79,14 @@ class KitchenVectorEnv(CtorPickle):
         self.tasks = tasks
         self.terminate_on_tasks_completed, self.remove_task_when_completed = terminate_on_tasks_completed, remove_task_when_completed
         self.object_noise_ratio, self.robot_noise_ratio = object_noise_ratio, robot_noise_ratio
-        self.num_envs, self.max_episode_steps, self.autoreset_mode = int(num_envs), max_episode_steps, autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
-        self.frame_skip = self.n_substeps = int(frame_skip)
+        self.frame_skip = int(frame_skip)
         # mesh_collision="hull": the nine Franka collision meshes collide through support maps on their reduced convex hulls (32 vertices
         # each; blob franka_kitchen_hull, kernels of csrc/b200sim_kitchen_hull.cu) instead of box proxies (DESIGN.md deviation 1)
         mesh_collision = kwargs.get("mesh_collision", "box")
         if mesh_collision not in ("box", "hull"):
             raise ValueError("mesh_collision must be 'box' or 'hull'")
         self.mesh_collision = mesh_collision
-        self.model = model if model is not None else load_model("franka_kitchen_hull" if mesh_collision == "hull" else "franka_kitchen")
-        m = self.model
-        self.task = make_kitchen_task(m, frame_skip)
+        m = model if model is not None else load_model("franka_kitchen_hull" if mesh_collision == "hull" else "franka_kitchen")
         # broadphase="groups" (default): the kernel build with the two-level broad phase (csrc/b200sim_kitchen_groups.cu) -- it
         # matches the flat-scan build bit for bit (tests/test_zz_kitchen_gpu.py) and tests far fewer pairs per sub-step; "flat": one
         # scan over all 3 708 pairs.  The library reads the choice from the
@@ -103,26 +97,28 @@ class KitchenVectorEnv(CtorPickle):
         if mesh_collision == "hull" and broadphase != "groups":
             raise ValueError("mesh_collision='hull' exists for the two-level broad phase only")
         self.broadphase = broadphase
-        prev = os.environ.get("B200SIM_KITCHEN_GROUPS")
-        os.environ["B200SIM_KITCHEN_GROUPS"] = "1" if broadphase == "groups" else "0"
-        try:
-            self.backend = (backend_factory or _KitchenBackend)(m, np.zeros((0, 11)), self.task, self.num_envs, device)
-        finally:
-            if prev is None:
-                del os.environ["B200SIM_KITCHEN_GROUPS"]
-            else:
-                os.environ["B200SIM_KITCHEN_GROUPS"] = prev
-        self.device = dev = self.backend.device
-        if rng_mode == "device":
-            raise NotImplementedError("rng_mode='device' (in-kernel reset draws, b200sim_reset) exists for the Fetch family only")
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)] \
-            if self.rng_mode == "numpy" else None
-        self._gen = torch.Generator(device=dev)
-        self._gen.seed()
-        lay = self.backend.layout
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu))}
-        self.dt = float(m.opt[0] * frame_skip)
+        factory = backend_factory or _KitchenBackend
+
+        def make_backend(*args):
+            prev = os.environ.get("B200SIM_KITCHEN_GROUPS")
+            os.environ["B200SIM_KITCHEN_GROUPS"] = "1" if broadphase == "groups" else "0"
+            try:
+                return factory(*args)
+            finally:
+                if prev is None:
+                    del os.environ["B200SIM_KITCHEN_GROUPS"]
+                else:
+                    os.environ["B200SIM_KITCHEN_GROUPS"] = prev
+
+        t = make_kitchen_task(m, frame_skip)
+        # `terminated` is the task bookkeeping below, not a kernel flag
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu)),
+                         action_space=Box(-1.0, 1.0, shape=(9,), dtype=np.float64),  # franka_env.py:90
+                         observation_space=Box(-np.inf, np.inf, shape=(int(t.nobs),), dtype=np.float64),
+                         backend_factory=make_backend, num_envs=num_envs, device=device, max_episode_steps=max_episode_steps,
+                         autoreset_mode=autoreset_mode, rng_mode=rng_mode, n_substeps=frame_skip, kwargs=kwargs)
+        self._can_terminate = bool(terminate_on_tasks_completed)
+        dev = self.device
         assert int(np.round(1.0 / self.dt)) == self.metadata["render_fps"]      # kitchen_env.py:311-313
         cfg = load_franka_config()                                              # franka_env.py:172-202
         nv = int(m.nv)
@@ -150,20 +146,11 @@ class KitchenVectorEnv(CtorPickle):
             idx_pad[j, :k], goal_pad[j, :k], live[j, :k] = OBS_ELEMENT_INDICES[t], OBS_ELEMENT_GOALS[t], 1.0
         self._idx_pad = torch.as_tensor(idx_pad.reshape(-1), device=dev)
         self._goal_pad, self._live_pad = f32(goal_pad), f32(live)
-        self._all_idx = torch.arange(self.num_envs, device=dev)
-        self.single_action_space = Box(-1.0, 1.0, shape=(9,), dtype=np.float64)  # franka_env.py:90
-        self.single_observation_space = Box(-np.inf, np.inf, shape=(int(self.task.nobs),), dtype=np.float64)
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
         n, k = self.num_envs, len(tasks)
-        self._elapsed = self.backend.elapsed                      # library-owned step counters (in-kernel TimeLimit)
-        self.backend.set_time_limit(max_episode_steps, False)     # `terminated` is the task bookkeeping below, not a kernel flag
-        self._needs_reset = torch.zeros(n, dtype=torch.bool, device=dev)
         self._todo = torch.ones((n, k), dtype=torch.bool, device=dev)            # tasks_to_complete
         self._episode_done = torch.zeros((n, k), dtype=torch.bool, device=dev)  # episode_task_completions
         self._last_robot_qpos = self.init_qpos[:9].expand(n, 9).clone()
-        self._last = None
-        self.closed = False
+        self._obs = torch.zeros((n, int(self.task.nobs)), dtype=torch.float32, device=dev)   # the noisy observation of the last call
 
     # ------------------------------------------------------------------ noise / observation
     def _noise(self, idx):
@@ -177,45 +164,37 @@ class KitchenVectorEnv(CtorPickle):
             u = torch.rand((n, self._noise_scale.numel()), generator=self._gen, device=self.device) * 2 - 1
         return u * self._noise_scale
 
-    def _obs_dict(self, out, obs):
+    def _obs_dict(self, out):
         q = out["achieved"]
-        return {"observation": obs,
-                "achieved_goal": {t: (q[:, self._run[t]] if self._run[t] is not None else q[:, self._idx[t]]) for t in self.tasks},
-                "desired_goal": {t: self._goal[t].expand(self.num_envs, -1) for t in self.tasks}}
+        return self._cast_obs({"observation": self._obs,
+                               "achieved_goal": {t: (q[:, self._run[t]] if self._run[t] is not None else q[:, self._idx[t]]) for t in self.tasks},
+                               "desired_goal": {t: self._goal[t].expand(self.num_envs, -1) for t in self.tasks}})
 
     # ------------------------------------------------------------------ reset
-    def _reset_envs(self, mask, out):
+    def _rest_record(self):
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
+        rest[self._sl["qpos"]] = self.init_qpos
+        rest[self._sl["qvel"]] = self.init_qvel
+        return rest
+
+    def _reset_envs(self, mask, out, options=None):
         """MujocoEnv.reset -> mj_resetData -> reset_model (franka_env.py:130-137), then KitchenEnv.reset (kitchen_env.py:425-437)."""
-        idx = torch.nonzero(mask, as_tuple=False).flatten()
+        idx = self._mask_indices(mask)
         if idx.numel() == 0:
-            return None
-        st, sl = self.backend.state, self._sl
-        rec = torch.zeros((idx.numel(), st.shape[1]), dtype=torch.float32, device=self.device)
-        rec[:, sl["qpos"]] = self.init_qpos
-        rec[:, sl["qvel"]] = self.init_qvel
-        st[idx] = rec
+            return
+        self.backend.state[idx] = self._rest.expand(idx.numel(), -1).clone()
         self._elapsed[idx] = 0
         self._todo[idx] = True
         self._episode_done[idx] = False
         self.backend.refresh(mask.to(torch.uint8), out)   # set_state -> mj_forward, noise-free observation
         noisy = out["obs"][idx] + self._noise(idx)
         self._last_robot_qpos[idx] = noisy[:, :9]
-        return idx, noisy
+        self._obs = self._obs.clone()
+        self._obs[idx] = noisy
 
-    def reset(self, *, seed=None, options=None):
-        if seed is not None:
-            seeds = [seed + i for i in range(self.num_envs)] if isinstance(seed, (int, np.integer)) else list(seed)
-            if self.rng_mode == "numpy":
-                self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(s))) for s in seeds]
-            self._gen.manual_seed(int(seeds[0]))
-        out = self.backend.new_outputs()
-        mask = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
-        _, noisy = self._reset_envs(mask, out)
-        self._needs_reset.zero_()
-        self._last = out
-        info = {"tasks_to_complete": self._todo.clone(), "episode_task_completions": self._episode_done.clone(),
+    def _reset_info(self, out):
+        return {"tasks_to_complete": self._todo.clone(), "episode_task_completions": self._episode_done.clone(),
                 "step_task_completions": torch.zeros_like(self._todo)}
-        return self._obs_dict(out, noisy), info
 
     # ------------------------------------------------------------------ step
     def control_targets(self, a):
@@ -224,18 +203,13 @@ class KitchenVectorEnv(CtorPickle):
         vel = torch.clamp(torch.clamp(a, -1.0, 1.0) * 2.0, self._vel_lo, self._vel_hi)
         return torch.clamp(self._last_robot_qpos + vel * self.dt, self._pos_lo, self._pos_hi).contiguous()
 
-    def step(self, actions):
-        if not torch.is_tensor(actions):
-            actions = torch.as_tensor(np.asarray(actions, dtype=np.float32))
-        if tuple(actions.shape) != (self.num_envs, 9):
-            raise ValueError("Action dimension mismatch")
-        a = actions.to(self.device, torch.float32, non_blocking=True)
-        ctrl = self.control_targets(a)
-        out = self.backend.new_outputs()
-        self.backend.step(ctrl, out)                                  # do_simulation(ctrl, 40) + TimeLimit: one kernel launch
-        truncated = out["truncated"]
-        obs = out["obs"] + self._noise(self._all_idx)
-        self._last_robot_qpos = obs[:, :9].clone()
+    def _kernel_input(self, actions):
+        return self.control_targets(actions)
+
+    def _step_results(self, out):
+        # the observation noise of every env is drawn before a NEXT_STEP reset draws its reset noise
+        self._obs = out["obs"] + self._noise(self._all_idx)
+        self._last_robot_qpos = self._obs[:, :9].clone()
         q = out["achieved"]
         # kitchen_env.py:356-369, 399-423
         # (|| q[task] - goal || < BONUS_THRESH for every task at once; the norm itself, as the reference compares it)
@@ -247,41 +221,25 @@ class KitchenVectorEnv(CtorPickle):
             self._todo = self._todo & ~step_done
         self._episode_done = self._episode_done | step_done
         terminated = self._episode_done.all(dim=1) if self.terminate_on_tasks_completed else torch.zeros_like(self._needs_reset)
-        info = {"tasks_to_complete": self._todo.clone(), "step_task_completions": step_done, "episode_task_completions": self._episode_done.clone()}
-        if self.autoreset_mode == "next_step" and bool(self._needs_reset.any()):
-            # envs that finished on the previous call are reset now; their action is ignored (gymnasium NEXT_STEP)
-            pre = self._needs_reset.clone()
-            idx, noisy = self._reset_envs(pre, out)
-            obs = obs.clone()
-            obs[idx] = noisy
-            reward = torch.where(pre, torch.zeros_like(reward), reward)
-            terminated = terminated & ~pre
-            truncated = truncated & ~pre
-            info = {"tasks_to_complete": self._todo.clone(), "step_task_completions": step_done & ~pre[:, None],
-                    "episode_task_completions": self._episode_done.clone()}
-            self._needs_reset.zero_()
-        done = terminated | truncated
-        if self.autoreset_mode == "next_step":
-            self._needs_reset = done
-        elif self.autoreset_mode == "same_step" and bool(done.any()):
-            info["final_obs"] = {k: (v.clone() if torch.is_tensor(v) else {kk: vv.clone() for kk, vv in v.items()})
-                                 for k, v in self._obs_dict(out, obs).items()}
-            info["_final_obs"] = done.clone()
-            idx, noisy = self._reset_envs(done, out)
-            obs = obs.clone()
-            obs[idx] = noisy
-        self._last = out
-        return self._obs_dict(out, obs), reward, terminated, truncated, info
+        info = {"tasks_to_complete": self._todo.clone(), "step_task_completions": step_done,
+                "episode_task_completions": self._episode_done.clone()}
+        return reward, terminated, out["truncated"], info
+
+    def _mask_results(self, out, pre, reward, terminated, truncated, info):
+        info = {"tasks_to_complete": self._todo.clone(), "step_task_completions": info["step_task_completions"] & ~pre[:, None],
+                "episode_task_completions": self._episode_done.clone()}
+        return torch.where(pre, torch.zeros_like(reward), reward), terminated & ~pre, truncated & ~pre, info
+
+    def _final_info(self, out, info, done):
+        return None   # the bookkeeping tensors of the step already describe the finished episodes
+
+    def _finish_info(self, out, info):
+        pass
 
     # GoalEnv-style reward on (achieved, desired) dicts of tensors: the number of listed tasks within BONUS_THRESH
     def compute_reward(self, achieved_goal, desired_goal, info=None):
         return sum((torch.linalg.norm(torch.as_tensor(achieved_goal[t]) - torch.as_tensor(desired_goal[t]), dim=-1) < BONUS_THRESH)
                    .to(torch.float32) for t in achieved_goal)
 
-    def get_state(self):
-        return self.backend.state.clone(), self._elapsed.clone()
-
-    def close(self):
-        if not getattr(self, "closed", True):
-            self.backend.close()
-            self.closed = True
+    def set_state(self, state, elapsed=None):
+        raise NotImplementedError("FrankaKitchen has no set_state: its noisy observation and last robot pose are not part of the record")

@@ -20,8 +20,8 @@ import torch
 from . import _lib
 from .fetch import CudaBackend
 from .models import load_model
-from .rollout import CtorPickle
-from .spaces import Box, Dict as DictSpace, batch_space
+from .spaces import Box, Dict as DictSpace
+from .vector import VectorEnv
 
 R, G, C = "r", "g", "c"
 MAPS = {
@@ -115,16 +115,15 @@ def make_antmaze_task(model, reward_type):
     return make_maze_task(model, reward_type, "ant")
 
 
-class _AntBackend(CudaBackend):
-    """CudaBackend of the maze agents (goal dim 2; the action dim comes from the task)."""
-
-
-class MazeVectorEnv(CtorPickle):
+class MazeVectorEnv(VectorEnv):
     """`gym.make_vec("AntMaze_Large-v5" | "PointMaze_UMaze-v3", num_envs=N)` replacement (torch CUDA tensors, leading
-    `num_envs` axis).  `maze_map` may be a name from `MAPS` or (for the point agent's tests) an explicit cell list."""
+    `num_envs` axis).  `maze_map` may be a name from `MAPS` or (for the point agent's tests) an explicit cell list.  The per-env
+    numpy streams exist in every rng_mode: explicit `options` cells and the goal update of `reset_target` draw from them."""
 
     metadata = {"render_modes": [], "render_fps": 50, "autoreset_mode": "next_step"}
     AGENT = "ant"
+    AUTO_RECOVER = False
+    SUCCESS_KEY = "success"
 
     def __init__(self, maze="Large", num_envs: int = 1, reward_type: str = "sparse", continuing_task: bool = True,
                  reset_target: bool = False, max_episode_steps: Optional[int] = None, device="cuda:0", rng_mode: str = "auto",
@@ -136,56 +135,35 @@ class MazeVectorEnv(CtorPickle):
             raise KeyError(f"unknown maze {maze!r}")
         if reward_type not in ("sparse", "dense"):
             raise ValueError("reward_type must be 'sparse' or 'dense'")
-        if kwargs.get("render_mode") is not None:
-            raise NotImplementedError("rendering is out of scope for the batched CUDA path")
-        if autoreset_mode not in ("next_step", "same_step", "disabled"):
-            raise ValueError("autoreset_mode must be next_step, same_step or disabled")
         self.maze_name, self.reward_type = maze, reward_type
         self.continuing_task, self.reset_target = continuing_task, reset_target
-        self.num_envs, self.autoreset_mode = int(num_envs), autoreset_mode
-        self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
         self.scaling, self.frame_skip = cfg["scaling"], cfg["frame_skip"]
-        self.metadata["render_fps"] = cfg["fps"]
         named = isinstance(maze, str)
-        self.max_episode_steps = (cfg["steps"][maze] if named else None) if max_episode_steps is None else max_episode_steps
         self.cells = MazeCells(MAPS[maze] if named else maze, cfg["scaling"])
         if model is None and not named:
             raise ValueError("an explicit maze map needs its compiled `model` (see models.compile_maze_model)")
-        self.model = model if model is not None else load_model(model_name(self.agent, maze))
+        m = model if model is not None else load_model(model_name(self.agent, maze))
         # Ant-v5 keyword [ext]: AntMaze_*-v5 observes the clipped per-body contact forces (ant_maze_v5.py:99: (105,) = 27 + 13 x 6);
         # AntMaze_*-v4 (Ant-v4, use_contact_forces False) and the point agent do not.  The registry sets it per id.
         self.include_cfrc = bool(include_cfrc_ext_in_observation) and self.agent == "ant"
-        self.task = make_maze_task(self.model, reward_type, self.agent, self.include_cfrc)
-        factory = backend_factory or _AntBackend
-        self.backend = factory(self.model, np.zeros((0, 11)), self.task, self.num_envs, device)
-        self.device = self.backend.device
-        # "device": goal / reset cells and their noise are drawn inside the library (b200sim_reset_maze, csrc/reset_sample.cuh)
-        self.rng_mode = rng_mode if rng_mode != "auto" else ("numpy" if self.num_envs <= 64 else "torch")
-        self.env_offset = int(kwargs.get("env_offset", 0))
-        self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(None))) for _ in range(self.num_envs)]
-        self._gen = torch.Generator(device=self.device)
-        self._gen.seed()
-        self._dev_seed = int(self._gen.initial_seed())
-        lay, m = self.backend.layout, self.model
-        self._sl = {k: slice(lay[k], lay[k] + n) for k, n in (("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 2))}
-        nobs = self.task.nobs
-        self.single_action_space = Box(-1.0, 1.0, shape=(m.nu,), dtype=np.float32)
-        self.single_observation_space = DictSpace(dict(
-            observation=Box(-np.inf, np.inf, shape=(nobs,), dtype=np.float64),
-            achieved_goal=Box(-np.inf, np.inf, shape=(2,), dtype=np.float64),
-            desired_goal=Box(-np.inf, np.inf, shape=(2,), dtype=np.float64)))
-        self.action_space = batch_space(self.single_action_space, self.num_envs)
-        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
+        t = make_maze_task(m, reward_type, self.agent, self.include_cfrc)
+        box = lambda n: Box(-np.inf, np.inf, shape=(n,), dtype=np.float64)
+        # "device": goal / reset cells and their noise are drawn inside the library (b200sim_reset_maze, csrc/reset_sample.cuh).
+        # TimeLimit and compute_terminated (maze_v4.py:390-398: success ends the episode unless continuing_task) run inside the
+        # step kernel
+        super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 2)),
+                         action_space=Box(-1.0, 1.0, shape=(m.nu,), dtype=np.float32),
+                         observation_space=DictSpace(dict(observation=box(t.nobs), achieved_goal=box(2), desired_goal=box(2))),
+                         backend_factory=backend_factory or CudaBackend, num_envs=num_envs, device=device,
+                         max_episode_steps=(cfg["steps"][maze] if named else None) if max_episode_steps is None else max_episode_steps,
+                         autoreset_mode=autoreset_mode, rng_mode=rng_mode, n_substeps=self.frame_skip, kwargs=kwargs,
+                         terminate_on_success=not continuing_task)
+        self.metadata["render_fps"] = cfg["fps"]
+        if self._np_rngs is None:
+            self._np_rngs = self._new_np_rngs([None] * self.num_envs)
         self.init_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)
         self._goal_loc = torch.as_tensor(self.cells.goal_locations, dtype=torch.float32, device=self.device)
         self._reset_loc = torch.as_tensor(self.cells.reset_locations, dtype=torch.float32, device=self.device)
-        # TimeLimit and compute_terminated (maze_v4.py:390-398: success ends the episode unless continuing_task) run inside the
-        # step kernel; the step counters are library memory
-        self._elapsed = self.backend.elapsed
-        self.backend.set_time_limit(self.max_episode_steps, not continuing_task)
-        self._needs_reset = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
-        self.dt = float(m.opt[0] * self.frame_skip)
-        self.closed = False
 
     # ------------------------------------------------------------------ sampling (MazeEnv.reset, maze_v4.py:299-358)
     def _noise_np(self, rng, xy):
@@ -229,15 +207,18 @@ class MazeVectorEnv(CtorPickle):
             bad = torch.linalg.norm(pos - goal, dim=1) <= 0.5 * self.scaling
         return goal, pos + (u(n, 2) * 2 - 1) * NOISE * self.scaling
 
+    def _rest_record(self):   # ant_env.init_qpos, zero velocities
+        rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
+        rest[self._sl["qpos"]] = self.init_qpos
+        return rest
+
     def _device_reset(self, mask, out):
-        if getattr(self, "_dev_reset", None) is None:
+        if self._dev_reset is None:
             from ._lib import MazeResetC
 
             p = MazeResetC()
             p.n_goal, p.n_reset, p.scaling, p.noise = len(self._goal_loc), len(self._reset_loc), float(self.scaling), float(NOISE)
-            rest = torch.zeros(self.backend.state.shape[1], dtype=torch.float32, device=self.device)
-            rest[self._sl["qpos"]] = self.init_qpos
-            self._dev_reset = (p, rest, self._goal_loc.contiguous(), self._reset_loc.contiguous())
+            self._dev_reset = (p, self._rest, self._goal_loc.contiguous(), self._reset_loc.contiguous())
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         p, rest, gl, rl = self._dev_reset
         self.backend.reset_maze(mask.to(torch.uint8), rest, p, gl, rl, self._dev_seed, self.env_offset, self._episode, out)
@@ -246,91 +227,41 @@ class MazeVectorEnv(CtorPickle):
     def _reset_envs(self, mask, out, options=None):
         if self.rng_mode == "device" and not options:   # explicit cells keep the reference-ordered host path
             return self._device_reset(mask, out)
-        idx = torch.nonzero(mask, as_tuple=False).flatten()
+        idx = self._mask_indices(mask)
         if idx.numel() == 0:
             return
         st, sl = self.backend.state, self._sl
         goal, pos = self._sample(idx, options)
-        rec = torch.zeros((idx.numel(), st.shape[1]), dtype=torch.float32, device=self.device)
-        rec[:, sl["qpos"]] = self.init_qpos          # ant_env.init_qpos with [:2] = reset_pos (ant_maze_v5.py:285)
-        rec[:, sl["qpos"].start: sl["qpos"].start + 2] = pos
+        rec = self._rest.expand(idx.numel(), -1).clone()
+        rec[:, sl["qpos"].start: sl["qpos"].start + 2] = pos    # ant_env.init_qpos with [:2] = reset_pos (ant_maze_v5.py:285)
         rec[:, sl["goal"]] = goal
         st[idx] = rec
         self._elapsed[idx] = 0
         self.backend.refresh(mask.to(torch.uint8), out)
 
     # ------------------------------------------------------------------ gymnasium API
-    def _obs_dict(self, out):
-        return self._cast_obs({"observation": out["obs"], "achieved_goal": out["achieved"], "desired_goal": out["desired"]})
+    def _reset_info(self, out):
+        return {"success": out["success"] > 0}
 
-    def reset(self, *, seed=None, options=None):
-        if seed is not None:
-            seeds = [seed + i for i in range(self.num_envs)] if isinstance(seed, (int, np.integer)) else list(seed)
-            self._np_rngs = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(s))) for s in seeds]
-            self._gen.manual_seed(int(seeds[0]))
-            self._dev_seed = int(seeds[0])
-            if getattr(self, "_episode", None) is not None:
-                self._episode.zero_()
-        out = self.backend.new_outputs()
-        self._reset_envs(torch.ones(self.num_envs, dtype=torch.bool, device=self.device), out, options)
-        self._needs_reset.zero_()
-        self._elapsed_ub, self._pending_reset = 0, False
-        self._last = out
-        return self._obs_dict(out), {"success": out["success"] > 0}
+    def _success(self, column):
+        return column > 0
 
-    def step(self, actions):
-        if not torch.is_tensor(actions):
-            actions = torch.as_tensor(np.asarray(actions, dtype=np.float32))
-        if tuple(actions.shape) != (self.num_envs, self.model.nu):
-            raise ValueError("Action dimension mismatch")
-        actions = actions.to(self.device, torch.float32, non_blocking=True).contiguous()
-        out = self.backend.new_outputs()
-        self.backend.step(actions, out)   # physics + observation + reward + success + terminated / truncated flags: one kernel
-        self._elapsed_ub = getattr(self, "_elapsed_ub", 0) + 1   # host-side upper bound of max(_elapsed)
-        reward, success = out["reward"], out["success"] > 0
-        terminated, truncated = out["terminated"], out["truncated"]
-        info = {"success": success, "solver_info": self.backend.info}
-        # a continuing task can only end by TimeLimit: then the host knows from its step counter when a check is due and
-        # does not synchronise with the device on the other steps
-        lazy = self.continuing_task
-        pre = None
-        if self.autoreset_mode == "next_step" and (not lazy or getattr(self, "_pending_reset", True)):
-            self._pending_reset = False
-            if bool(self._needs_reset.any()):
-                # envs that finished on the previous call are reset now: their action was ignored, so the step they did not
-                # take reports reward 0, no success and no flags (gymnasium NEXT_STEP)
-                pre = self._needs_reset.clone()
-                self._reset_envs(pre, out)
-                k = self.backend.nobs + 2 * self.backend.ngoal
-                out["packed"][:, k:k + 4].masked_fill_(pre[:, None], 0.0)
-                out["flags"].masked_fill_(pre[None, :], 0)
-                success = success & ~pre
-                info["success"] = success
-                self._needs_reset.zero_()
-                self._elapsed_ub = int(self._elapsed.max())
+    def _step_results(self, out):
+        reward, terminated, truncated, info = super()._step_results(out)
+        info["success"] = self._success(out["success"])
+        return reward, terminated, truncated, info
+
+    def _mask_results(self, out, pre, reward, terminated, truncated, info):
+        info["success"] = info["success"] & ~pre
+        return super()._mask_results(out, pre, reward, terminated, truncated, info)
+
+    def _after_autoreset(self, out, info):
+        success = info["success"]
         if self.continuing_task and self.reset_target and len(self.cells.goal_locations) > 1 and bool(success.any()):
             self._update_goal(success, out)  # maze_v4.py:400-418 (never for the envs that were just reset: `success` is masked)
-        may_truncate = self.max_episode_steps is not None and (not lazy or self._elapsed_ub >= self.max_episode_steps)
-        if may_truncate or not lazy:
-            done = truncated | terminated
-            if self.autoreset_mode == "next_step":
-                self._needs_reset = done
-                self._pending_reset = True
-            elif self.autoreset_mode == "same_step":
-                if bool(done.any()):
-                    info["final_obs"] = {k: v.clone() for k, v in self._obs_dict(out).items()}
-                    info["_final_obs"] = done.clone()
-                    # gymnasium's SAME_STEP convention: the info of the finished episodes next to their last observation
-                    info["final_info"] = {"success": success.clone(), "_success": done.clone()}
-                    info["_final_info"] = done.clone()
-                    self._reset_envs(done, out)
-                self._elapsed_ub = int(self._elapsed.max())
-        self._last = out      # the packed rows of this step (obs | achieved | desired | reward | success | flags)
-        return self._obs_dict(out), reward, terminated, truncated, info
 
-    @property
-    def solver_overflow_count(self):
-        return int(self.backend.overflow_counter[0])
+    def _finish_info(self, out, info):
+        pass   # `success` as of the step, before a SAME_STEP reset; no mask entry
 
     def _update_goal(self, success, out):
         idx = torch.nonzero(success, as_tuple=False).flatten()
@@ -343,37 +274,13 @@ class MazeVectorEnv(CtorPickle):
                 goal = self._noise_np(rng, self.cells.goal_locations[rng.integers(low=0, high=len(self.cells.goal_locations))].copy())
             st[i, sl["goal"]] = torch.as_tensor(goal, dtype=torch.float32, device=self.device)
 
-    def compute_reward(self, achieved_goal, desired_goal, info=None):
-        is_np = not torch.is_tensor(achieved_goal)
-        ag = torch.as_tensor(np.asarray(achieved_goal)) if is_np else achieved_goal
-        dg = torch.as_tensor(np.asarray(desired_goal)) if not torch.is_tensor(desired_goal) else desired_goal
-        r = self.backend.compute_reward(ag, dg).reshape(ag.shape[:-1])
-        return r.cpu().numpy().astype(np.float64) if is_np else r
+    def _reward_np_dtype(self):
+        return np.float64
 
     def compute_terminated(self, achieved_goal, desired_goal, info=None):
         if not self.continuing_task:
             return bool(np.linalg.norm(np.asarray(achieved_goal) - np.asarray(desired_goal)) <= SUCCESS_RADIUS)
         return False
-
-    def compute_truncated(self, achieved_goal, desired_goal, info=None):
-        return False
-
-    def get_state(self):
-        return self.backend.state.clone(), self._elapsed.clone()
-
-    def set_state(self, state, elapsed=None):
-        self.backend.state.copy_(state)
-        if elapsed is not None:
-            self._elapsed.copy_(elapsed)
-        self._elapsed_ub = int(self._elapsed.max())
-        out = self.backend.new_outputs()
-        self.backend.refresh(None, out)
-        return self._obs_dict(out)
-
-    def close(self):
-        if not getattr(self, "closed", True):
-            self.backend.close()
-            self.closed = True
 
 
 class AntMazeVectorEnv(MazeVectorEnv):

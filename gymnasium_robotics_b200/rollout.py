@@ -72,7 +72,7 @@ class CtorPickle:
         dt = getattr(self, "obs_dtype", None)
         if dt is None:
             return obs
-        return {k: v.to(dt) for k, v in obs.items()} if isinstance(obs, dict) else obs.to(dt)
+        return {k: self._cast_obs(v) for k, v in obs.items()} if isinstance(obs, dict) else obs.to(dt)   # (the kitchen's goals nest)
 
     def render(self):
         return None   # rendering is out of scope for the batched CUDA path (render_mode is always None)
