@@ -19,7 +19,7 @@ import torch
 
 from . import _lib
 from .fetch import CudaBackend
-from .models import load_model
+from .models import build_maze_model, load_model
 from .spaces import Box, Dict as DictSpace
 from .vector import VectorEnv
 
@@ -97,6 +97,33 @@ class MazeCells:
         return np.array([math.floor((self.y_center - xy[1]) / self.scaling), math.floor((xy[0] + self.x_center) / self.scaling)])
 
 
+def check_maze_map(maze_map, scaling):
+    """The cells of a user layout (`maze_map=`) as a list of rows, or ValueError with the reason.  Beyond the reference, a
+    layout is refused when some goal location has no reset location in another cell: the reference's start draw
+    (`generate_reset_pos`, maze_v4.py:276-297) would loop forever on it, and the device draw (csrc/reset_sample.cuh) would give up and start the env
+    in its goal cell."""
+    try:
+        rows = [list(row) for row in maze_map]
+    except TypeError:
+        raise ValueError("maze_map must be a list of rows of cells") from None
+    if not rows or not rows[0]:
+        raise ValueError("maze_map is empty")
+    if any(len(row) != len(rows[0]) for row in rows):
+        raise ValueError(f"maze_map is not rectangular: row lengths {[len(row) for row in rows]}")
+    for i, row in enumerate(rows):
+        for j, cell in enumerate(row):
+            if not (cell in (R, G, C) if isinstance(cell, str) else
+                    (isinstance(cell, (int, np.integer)) and not isinstance(cell, bool) and cell in (0, 1))):
+                raise ValueError(f"maze_map[{i}][{j}] = {cell!r}: a cell is 0, 1, {R!r}, {G!r} or {C!r}")
+    cells = MazeCells(rows, scaling)
+    if len(cells.goal_locations) == 0 or len(cells.reset_locations) == 0:
+        raise ValueError(f"maze_map has no {'goal' if len(cells.goal_locations) == 0 else 'reset'} location")
+    for g in cells.goal_locations:
+        if not bool((np.linalg.norm(cells.reset_locations - g, axis=1) > 0.5 * scaling).any()):
+            raise ValueError(f"maze_map: the goal cell {tuple(cells.cell_xy_to_rowcol(g).tolist())} has no reset location in another cell")
+    return rows
+
+
 def make_maze_task(model, reward_type, agent="ant", contact_forces=False):
     """contact_forces: append Ant-v5's clipped `cfrc_ext[1:]` (6 values per body) to the observation -- (105,) instead of (27,)"""
     cfg = AGENTS[agent]
@@ -117,8 +144,11 @@ def make_antmaze_task(model, reward_type):
 
 class MazeVectorEnv(VectorEnv):
     """`gym.make_vec("AntMaze_Large-v5" | "PointMaze_UMaze-v3", num_envs=N)` replacement (torch CUDA tensors, leading
-    `num_envs` axis).  `maze_map` may be a name from `MAPS` or (for the point agent's tests) an explicit cell list.  The per-env
-    numpy streams exist in every rng_mode: explicit `options` cells and the goal update of `reset_target` draw from them."""
+    `num_envs` axis).  `maze` is a name from `MAPS` or (for the point agent's tests) an explicit cell list with its compiled
+    `model`.  `maze_map=` is the reference's custom layout (point_maze.py:195-207, ant_maze_v5.py:221-229): a list of rows of
+    0, 1, "r", "g", "c" cells (`check_maze_map`), built on the agent's committed model (`models.build_maze_model`) unless a
+    `model` is given; the named `maze` still supplies the episode length.  The per-env numpy streams exist in every rng_mode:
+    explicit `options` cells and the goal update of `reset_target` draw from them."""
 
     metadata = {"render_modes": [], "render_fps": 50, "autoreset_mode": "next_step"}
     AGENT = "ant"
@@ -128,7 +158,7 @@ class MazeVectorEnv(VectorEnv):
     def __init__(self, maze="Large", num_envs: int = 1, reward_type: str = "sparse", continuing_task: bool = True,
                  reset_target: bool = False, max_episode_steps: Optional[int] = None, device="cuda:0", rng_mode: str = "auto",
                  autoreset_mode: str = "next_step", backend_factory=None, agent: Optional[str] = None, model=None,
-                 include_cfrc_ext_in_observation: bool = False, **kwargs):
+                 include_cfrc_ext_in_observation: bool = False, maze_map=None, **kwargs):
         self.agent = agent or self.AGENT
         cfg = AGENTS[self.agent]
         if isinstance(maze, str) and maze not in MAPS:
@@ -139,10 +169,19 @@ class MazeVectorEnv(VectorEnv):
         self.continuing_task, self.reset_target = continuing_task, reset_target
         self.scaling, self.frame_skip = cfg["scaling"], cfg["frame_skip"]
         named = isinstance(maze, str)
-        self.cells = MazeCells(MAPS[maze] if named else maze, cfg["scaling"])
+        if maze_map is not None:
+            if not named:
+                raise ValueError("give the layout once: as `maze_map=` or as an explicit `maze` cell list, not both")
+            layout = check_maze_map(maze_map, cfg["scaling"])
+        else:
+            layout = MAPS[maze] if named else maze
+        self.cells = MazeCells(layout, cfg["scaling"])
         if model is None and not named:
             raise ValueError("an explicit maze map needs its compiled `model` (see models.compile_maze_model)")
-        m = model if model is not None else load_model(model_name(self.agent, maze))
+        if model is not None:
+            m = model
+        else:
+            m = build_maze_model(self.agent, layout) if maze_map is not None else load_model(model_name(self.agent, maze))
         # Ant-v5 keyword [ext]: AntMaze_*-v5 observes the clipped per-body contact forces (ant_maze_v5.py:99: (105,) = 27 + 13 x 6);
         # AntMaze_*-v4 (Ant-v4, use_contact_forces False) and the point agent do not.  The registry sets it per id.
         self.include_cfrc = bool(include_cfrc_ext_in_observation) and self.agent == "ant"

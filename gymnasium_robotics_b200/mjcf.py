@@ -742,27 +742,98 @@ def _dense_mass_matrix(nbody, nv, parent, mass, inertia, xipos, ximat, xmat, joi
     return M, jacs
 
 
+def maze_walls(maze_map, maze_size_scaling, maze_height):
+    """The geometry part of `Maze.make_maze` (gymnasium_robotics/envs/maze/maze_v4.py:148-242): one static box per wall cell,
+    as (name, centre, half extents) in row-major order on a grid centred at the origin, and the wall grid of the step kernel's
+    wall lookup."""
+    length, width = len(maze_map), len(maze_map[0])
+    xc, yc = width / 2 * maze_size_scaling, length / 2 * maze_size_scaling
+    half = (0.5 * maze_size_scaling, 0.5 * maze_size_scaling, maze_height / 2 * maze_size_scaling)
+    walls = [(f"block_{i}_{j}", ((j + 0.5) * maze_size_scaling - xc, yc - (i + 0.5) * maze_size_scaling, half[2]), half)
+             for i in range(length) for j in range(width) if maze_map[i][j] == 1]
+    grid = dict(length=length, width=width, scaling=float(maze_size_scaling), height=float(maze_height),
+                walls=[[1 if maze_map[i][j] == 1 else 0 for j in range(width)] for i in range(length)])
+    return walls, grid
+
+
 def make_maze_xml(agent_xml_path, maze_map, maze_size_scaling, maze_height):
-    """MJCF tree of an agent placed in a maze: restates the geometry part of `Maze.make_maze`
-    (gymnasium_robotics/envs/maze/maze_v4.py:148-242): one static box per wall cell, centred grid, target site."""
+    """MJCF tree of an agent placed in a maze: the agent's MJCF, the wall boxes of `maze_walls` and the target site."""
     tree = ET.parse(agent_xml_path)
     root = tree.getroot()
     worldbody = root.find(".//worldbody")
-    length, width = len(maze_map), len(maze_map[0])
-    xc, yc = width / 2 * maze_size_scaling, length / 2 * maze_size_scaling
-    for i in range(length):
-        for j in range(width):
-            if maze_map[i][j] == 1:
-                x = (j + 0.5) * maze_size_scaling - xc
-                y = yc - (i + 0.5) * maze_size_scaling
-                ET.SubElement(worldbody, "geom", name=f"block_{i}_{j}", pos=f"{x} {y} {maze_height / 2 * maze_size_scaling}",
-                              size=f"{0.5 * maze_size_scaling} {0.5 * maze_size_scaling} {maze_height / 2 * maze_size_scaling}",
-                              type="box", contype="1", conaffinity="1")
+    walls, grid = maze_walls(maze_map, maze_size_scaling, maze_height)
+    for name, pos, size in walls:
+        ET.SubElement(worldbody, "geom", name=name, pos=" ".join(map(str, pos)), size=" ".join(map(str, size)),
+                      type="box", contype="1", conaffinity="1")
     ET.SubElement(worldbody, "site", name="target", pos=f"0 0 {maze_height / 2 * maze_size_scaling}",
                   size=f"{0.2 * maze_size_scaling}", type="sphere")
-    grid = dict(length=length, width=width, scaling=float(maze_size_scaling), height=float(maze_height),
-                walls=[[1 if maze_map[i][j] == 1 else 0 for j in range(width)] for i in range(length)])
     return root, grid
+
+
+def _grid_tables(grid, pair_geom2_names):
+    """pair_grid, grid_dims, grid_walls, grid_param: a pair whose second geom is a maze wall block is served by the step
+    kernel's grid lookup instead of the pair list."""
+    pair_grid = np.array([1 if (grid is not None and n.startswith("block_")) else 0 for n in pair_geom2_names], dtype=np.int32)
+    if grid is None:
+        return pair_grid, np.zeros(2, dtype=np.int32), np.zeros(0, dtype=np.int32), np.zeros(4)
+    return (pair_grid, np.array([grid["length"], grid["width"]], dtype=np.int32), np.array(grid["walls"], dtype=np.int32).ravel(),
+            np.array([grid["scaling"], grid["height"], grid["width"] / 2 * grid["scaling"], grid["length"] / 2 * grid["scaling"]]))
+
+
+def _geom_rbound(typ, size, hull=None):
+    """Bounding-sphere radius of a runtime geom about its centre."""
+    return {GEOM_PLANE: 0.0, GEOM_SPHERE: size[0], GEOM_CAPSULE: size[0] + size[1], GEOM_CYLINDER: np.hypot(size[0], size[1]),
+            GEOM_BOX: np.linalg.norm(size), GEOM_ELLIPSOID: max(size),
+            GEOM_MESH: (float(np.linalg.norm(hull, axis=1).max()) if hull is not None else 0.0)}[typ]
+
+
+def replace_maze_walls(model, maze_map, maze_size_scaling, maze_height) -> "Model":
+    """The compiled agent-in-a-maze `model` with its walls replaced by those of `maze_map`: the model `compile_mjcf` makes of
+    `make_maze_xml` on that map, without the agent's MJCF.
+
+    All wall blocks are world geoms with the same attributes, so the model's own wall pairs give each agent geom's contact
+    parameters against any wall.  compile_mjcf lists the wall blocks last (they are the last geoms of the MJCF) and the
+    dynamic pairs in the order of its candidate loop, by (lower geom index, higher geom index); the new pair list keeps that
+    order.  The target site does not depend on the layout and stays."""
+    m = Model.from_blob(model.to_blob())
+    names = m.names["geom"]
+    wall = np.array([n.startswith("block_") for n in names], dtype=bool)
+    na = len(names) - int(wall.sum())
+    if not wall.any() or wall[:na].any() or m.geom_hull.size:
+        raise ValueError("not a compiled maze model: its wall blocks must be its last geoms")
+    if not np.array_equal(m.site_pos[m.site_id("target")], [0.0, 0.0, maze_height / 2 * maze_size_scaling]):
+        raise ValueError("the model's maze has another scaling or height")
+    keys = [(min(a, b), max(a, b)) for a, b in zip(m.pair_geom1.tolist(), m.pair_geom2.tolist())]
+    if keys != sorted(keys):
+        raise ValueError("the model has explicit contact pairs: its wall pairs cannot be rebuilt")
+    walls, grid = maze_walls(maze_map, maze_size_scaling, maze_height)
+    rows, template = [], {}    # rows: (lower geom, higher geom, geom1, geom2, pair row that carries the parameters)
+    for k, (a, b) in enumerate(zip(m.pair_geom1.tolist(), m.pair_geom2.tolist())):
+        if wall[a] or wall[b]:
+            template.setdefault(b if wall[a] else a, (k, bool(wall[a])))
+        else:
+            rows.append((*keys[k], a, b, k))
+    for a, (k, wall_first) in template.items():
+        for w in range(na, na + len(walls)):
+            rows.append((a, w, w, a, k) if wall_first else (a, w, a, w, k))
+    rows.sort()
+    src = np.array([r[4] for r in rows], dtype=np.int64)
+    m.pair_geom1, m.pair_geom2 = np.array([r[2] for r in rows], dtype=np.int32), np.array([r[3] for r in rows], dtype=np.int32)
+    for f in ("pair_condim", "pair_friction", "pair_margin", "pair_gap", "pair_solref", "pair_solimp", "pair_invweight"):
+        setattr(m, f, getattr(m, f)[src])
+    nw = len(walls)
+    m.geom_type = np.concatenate([m.geom_type[:na], np.full(nw, GEOM_BOX, dtype=np.int32)])
+    m.geom_body = np.concatenate([m.geom_body[:na], np.zeros(nw, dtype=np.int32)])
+    m.geom_mjbody = np.concatenate([m.geom_mjbody[:na], np.zeros(nw, dtype=np.int32)])
+    m.geom_pos = np.concatenate([m.geom_pos[:na], np.array([p for _, p, _ in walls]).reshape(-1, 3)])
+    m.geom_quat = np.concatenate([m.geom_quat[:na], np.tile([1.0, 0, 0, 0], (nw, 1))])
+    m.geom_size = np.concatenate([m.geom_size[:na], np.array([s for _, _, s in walls]).reshape(-1, 3)])
+    m.geom_rbound = np.concatenate([m.geom_rbound[:na], [_geom_rbound(GEOM_BOX, np.array(s)) for _, _, s in walls]])
+    m.names["geom"] = names[:na] + [n for n, _, _ in walls]
+    m.pair_grid, m.grid_dims, m.grid_walls, m.grid_param = _grid_tables(grid, [m.names["geom"][g] for g in m.pair_geom2])
+    m.sizes[Model.SIZES.index("ngeom")], m.sizes[Model.SIZES.index("npair")] = na + nw, len(rows)
+    m._reshape()
+    return m
 
 
 def compile_mjcf(path, overrides=None, mesh_mesh=False, root=None, grid=None, mesh_hull=False) -> Model:
@@ -986,10 +1057,7 @@ def compile_mjcf(path, overrides=None, mesh_mesh=False, root=None, grid=None, me
         gp.append(rel_pos[b] + qrot(rel_quat[b], pos))
         gq.append(qmul(rel_quat[b], quat))
         gs.append(size)
-        gr.append({GEOM_PLANE: 0.0, GEOM_SPHERE: size[0], GEOM_CAPSULE: size[0] + size[1],
-                   GEOM_CYLINDER: np.hypot(size[0], size[1]), GEOM_BOX: np.linalg.norm(size),
-                   GEOM_ELLIPSOID: max(size),
-                   GEOM_MESH: (float(np.linalg.norm(hull, axis=1).max()) if hull is not None else 0.0)}[typ])
+        gr.append(_geom_rbound(typ, size, hull))
     m.geom_type, m.geom_body = np.array(gt, dtype=np.int32), np.array(gb, dtype=np.int32)
     if hverts:     # optional blob fields (absent from models without hull geoms: their blobs do not change)
         m.geom_hull, m.hull_vert = np.array(ghull, dtype=np.int32).reshape(-1, 2), np.array(hverts, dtype=np.float64).reshape(-1, 3)
@@ -1065,15 +1133,8 @@ def compile_mjcf(path, overrides=None, mesh_mesh=False, root=None, grid=None, me
                  floats(pr.get("solref"), 2, None) if pr.get("solref") else 0.5 * (g1["solref"] + g2["solref"]),
                  floats(pr.get("solimp"), 5, [0.9, 0.95, 0.001, 0.5, 2]) if pr.get("solimp") else 0.5 * (g1["solimp"] + g2["solimp"]))
     m.pair_geom1, m.pair_geom2, m.pair_condim = (np.array(x, dtype=np.int32) for x in (P1, P2, PC))
-    # maze walls: pairs whose second geom is a wall block can be served by a grid lookup instead of the pair list
     gnames = [F.geoms[g]["name"] for g in gkeep]
-    m.pair_grid = np.array([1 if (grid is not None and gnames[b].startswith("block_")) else 0 for b in P2], dtype=np.int32)
-    if grid is not None:
-        m.grid_dims = np.array([grid["length"], grid["width"]], dtype=np.int32)
-        m.grid_walls = np.array(grid["walls"], dtype=np.int32).ravel()
-        m.grid_param = np.array([grid["scaling"], grid["height"], grid["width"] / 2 * grid["scaling"], grid["length"] / 2 * grid["scaling"]])
-    else:
-        m.grid_dims, m.grid_walls, m.grid_param = np.zeros(2, dtype=np.int32), np.zeros(0, dtype=np.int32), np.zeros(4)
+    m.pair_grid, m.grid_dims, m.grid_walls, m.grid_param = _grid_tables(grid, [gnames[b] for b in P2])
     m.pair_friction = np.array(PF).reshape(-1, 5)
     m.pair_margin, m.pair_gap = np.array(PM), np.array(PG)
     m.pair_solref, m.pair_solimp, m.pair_invweight = np.array(PSR).reshape(-1, 2), np.array(PSI).reshape(-1, 5), np.array(PIW).reshape(-1, 2)

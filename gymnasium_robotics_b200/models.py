@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import os
 
-from .mjcf import Model, compile_mjcf
+from .mjcf import Model, compile_mjcf, replace_maze_walls
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 MODEL_DIR = os.path.join(_HERE, "models")
@@ -62,13 +62,23 @@ MAZE_MODELS = {f"{a}maze_{k.lower()}": (a, k) for a in ("ant", "point") for k in
 
 
 def compile_maze_model(agent, maze_map):
-    """Compile agent + maze walls (restating Maze.make_maze, maze_v4.py:148-242); needs the reference assets."""
+    """Compile agent + maze walls (restating Maze.make_maze, maze_v4.py:148-242); needs the reference assets.  Generates the
+    committed maze blobs; the envs build custom layouts with `build_maze_model`."""
     from .maze import AGENTS
     from .mjcf import make_maze_xml
 
     xml = os.path.normpath(os.path.join(REFERENCE_ASSETS, ANT_XML if agent == "ant" else POINT_XML))
     root, grid = make_maze_xml(xml, maze_map, AGENTS[agent]["scaling"], AGENTS[agent]["height"])
     return compile_mjcf(xml, root=root, grid=grid)
+
+
+def build_maze_model(agent, maze_map):
+    """The model of `agent` ("ant" or "point") in the layout `maze_map`, equal to `compile_maze_model(agent, maze_map)` but
+    built from the committed U-maze blob of the same agent (`mjcf.replace_maze_walls`), so it needs no reference assets."""
+    from .maze import AGENTS
+
+    cfg = AGENTS[agent]
+    return replace_maze_walls(load_model(f"{agent}maze_umaze"), maze_map, cfg["scaling"], cfg["height"])
 
 
 def build_models(force: bool = False):
