@@ -73,9 +73,14 @@ struct Ctx {
 enum { TM_KIN = 0, TM_COM_M, TM_COLL, TM_CONSTR, TM_SMOOTH, TM_NBEGIN, TM_NCHECK, TM_BUILDH, TM_NDIR, TM_NMOVE, TM_INTEG, TM_BARRIER, TM_OTHER, TM_MV_MULM, TM_MV_ROWS, TM_MV_LS, TM_CK_PASSF, TM_MV_UPD, TM_COUNT };
 #define TIC() long long t0_ = clock64()
 #define TOC(k) do { long long t1_ = clock64(); c.tim[k] += t1_ - t0_; t0_ = t1_; } while (0)
+// the convergence check ends newton_begin and newton_move: its cycles move from that stage's counter to TM_NCHECK
+#define CHECK_TIC() long long tc_ = clock64()
+#define CHECK_TOC(stage) do { long long d_ = clock64() - tc_; c.tim[TM_NCHECK] += d_; c.tim[stage] -= d_; } while (0)
 #else
 #define TIC() do { } while (0)
 #define TOC(k) do { } while (0)
+#define CHECK_TIC() do { } while (0)
+#define CHECK_TOC(stage) do { } while (0)
 #endif
 #ifdef __CUDACC__
 // the step kernel's dynamic shared memory (`smem` in step_kernel.cuh): model header + HOT arrays, then one scratch per warp
@@ -1454,8 +1459,11 @@ HD void con_w(const float* cr, int k, float* w) {
 }
 HD float con_mu(const float* cr, int k) { return k < 3 ? cr[C_MU] : cr[C_MU + 1]; }  // base row k >= 1
 #endif
+// C_DIMGRP: condim (8 bits), group (8 bits), and from the solver's first check on the activity of the contact's edges at the
+// current point (bit 0: u_n < 0 of a frictionless contact; pyramid: bit 2 (k - 1) u_n + mu u_k < 0, bit 2 (k - 1) + 1 u_n - mu u_k < 0)
 HD int con_dim(const float* cr) { return ((const int*)cr)[C_DIMGRP] & 0xff; }
-HD int con_grp(const float* cr) { return ((const int*)cr)[C_DIMGRP] >> 8; }
+HD int con_grp(const float* cr) { return (((const int*)cr)[C_DIMGRP] >> 8) & 0xff; }
+HD uint32_t con_act(const float* cr) { return ((const uint32_t*)cr)[C_DIMGRP] >> 16; }
 
 template <bool HF>
 STAGE void make_constraint(const Ctx c) {
@@ -1623,6 +1631,44 @@ STAGE void make_constraint(const Ctx c) {
   if (HF) { LANES(d, h->nfric) SF(fric)[d] = 0.f; SYNC(); }
 }
 
+// base-row generalized forces of a contact from its base-row values U (pyramid edges f = -D * min(0, u_n +- mu u_k)).  Returns
+// the activity of the edges, in the layout of con_act(): the solver stores it in the record for build_H.
+HD uint32_t contact_base_forces(const float* cr, int dim, const float (&U)[C_NB], float* F) {
+  float D = cr[C_D], un = U[0];
+#pragma unroll
+  for (int k = 0; k < C_NB; k++) F[k] = 0;
+  if (dim == 1) { F[0] = un < 0 ? -D * un : 0.f; return un < 0 ? 1u : 0u; }
+  uint32_t act = 0;
+#pragma unroll
+  for (int k = 1; k < C_NB; k++) {   // (statically indexed so that U and F stay in registers)
+    if (k >= dim) continue;
+    float mu = con_mu(cr, k), uk = U[k];
+    float xp = un + mu * uk, xm = un - mu * uk;
+    float fp = xp < 0 ? -D * xp : 0.f, fm = xm < 0 ? -D * xm : 0.f;
+    act |= (xp < 0 ? 1u : 0u) << (2 * k - 2) | (xm < 0 ? 1u : 0u) << (2 * k - 1);
+    F[0] += fp + fm;
+    F[k] = mu * (fp - fm);
+  }
+  return act;
+}
+// the same from the values stored in the record
+HD void contact_base_forces(const float* cr, int dim, float* F) {
+  float U[C_NB];
+#pragma unroll
+  for (int k = 0; k < C_NB; k++) U[k] = cr[C_U + k];
+  contact_base_forces(cr, dim, U, F);
+}
+// the solver's contact update: the base-row forces of the new values U parked in the JV slots (read by pass_F, rewritten by the
+// next J * search product) and the edge activity in the record (read by build_H)
+HD void contact_park_forces(float* cr, const float (&U)[C_NB]) {
+  int* dg = (int*)cr + C_DIMGRP;
+  float F[C_NB];
+  const uint32_t act = contact_base_forces(cr, *dg & 0xff, U, F);
+#pragma unroll
+  for (int k = 0; k < C_NB; k++) cr[C_JV + k] = F[k];
+  *dg = (int)(((uint32_t)*dg & 0xffffu) | act << 16);
+}
+
 // JV slots of every row <- J * vec (the search direction); the opening passes J qvel / J qacc are fused in rows_begin()
 template <bool HF>
 STAGE void rows_from_vec(const Ctx c, const float* vec) {
@@ -1697,14 +1743,20 @@ STAGE void rows_begin(const Ctx c, const float* qvel, const float* qacc) {
     const float* gr = SF(group) + con_grp(cr) * GRP_WORDS;
     const float* gA = dA + 6 * con_grp(cr);
     float Bc = cr[C_JV];
-    for (int k = 0; k < nbase; k++) {
+    float U[C_NB];
+#pragma unroll
+    for (int k = 0; k < C_NB; k++) {   // (statically indexed so that U stays in registers)
+      U[k] = 0.f;
+      if (k >= nbase) continue;
       float w[6];
       con_w(cr, k, w);
       float u = cr[C_U + k];
       u += Bc * dot6(w, gr + G_V);
       u += dot6(w, gA);
       cr[C_U + k] = u;
+      U[k] = u;
     }
+    contact_park_forces(cr, U);   // for the solver's first check (Bc is not read again)
   }
   LANES(i, cnt[CNT_NWELD] * 6) {
     float* wr = SF(weld) + (i / 6) * WELD_WORDS;
@@ -1738,42 +1790,16 @@ STAGE void rows_begin(const Ctx c, const float* qvel, const float* qacc) {
 
 // ---------------------------------------------------------------------------------------------------------------
 // 8. Newton solver pieces
-// base-row generalized forces of a contact from its base-row values U (pyramid edges f = -D * min(0, u_n +- mu u_k))
-HD void contact_base_forces(const float* cr, int dim, float* F) {
-  float D = cr[C_D], un = cr[C_U];
-#pragma unroll
-  for (int k = 0; k < C_NB; k++) F[k] = 0;
-  if (dim == 1) { F[0] = un < 0 ? -D * un : 0.f; return; }
-#pragma unroll
-  for (int k = 1; k < C_NB; k++) {   // (statically indexed so that F stays in registers)
-    if (k >= dim) continue;
-    float mu = con_mu(cr, k), uk = cr[C_U + k];
-    float xp = un + mu * uk, xm = un - mu * uk;
-    float fp = xp < 0 ? -D * xp : 0.f, fm = xm < 0 ? -D * xm : 0.f;
-    F[0] += fp + fm;
-    F[k] = mu * (fp - fm);
-  }
-}
-
-// fcon = J^T f from the stored base-row forces: per-group spatial force, then one 6-dot per (dof, group)
+// fcon = J^T f from the base-row forces that the contact update parked in the JV slots (contact_park_forces, followed by a
+// SYNC): per-group spatial force, then one 6-dot per (dof, group)
 template <bool HF>
-STAGE void pass_F(const Ctx c, float* out) {
+HD void pass_F(const Ctx c, float* out) {
+  // (no ASSUME_SHARED_PTR(out): with it, nvcc 12.9 compiled the check inlined into newton_begin / newton_move as unreachable
+  // and dropped it; tests/test_newton_fused_check.py looks for the check in both)
   ASSUME_SHARED(c);
-  ASSUME_SHARED_PTR(out);
   const DMHead* h = c.h;
   const int* cnt = SI(counters);
   int ngrp = cnt[CNT_NGRP], nweld = cnt[CNT_NWELD], ndr = cnt[CNT_NDR];
-  // base-row forces once per contact (parked in the JV slots, which are rewritten by the next J * search product)
-  LANES(i, cnt[CNT_NCON]) {
-    float* cr = SF(con) + i * CON_WORDS;
-    float F[C_NB];
-    contact_base_forces(cr, con_dim(cr), F);
-    cr[C_JV] = F[0]; cr[C_JV + 1] = F[1]; cr[C_JV + 2] = F[2]; cr[C_JV + 3] = F[3];
-#ifdef B200_KITCHEN
-    cr[C_JV + 4] = F[4]; cr[C_JV + 5] = F[5];
-#endif
-  }
-  SYNC();
   LANES(idx, ngrp * 6) {
     int g = idx / 6, a = idx - 6 * g;
     float* gr = SF(group) + g * GRP_WORDS;
@@ -1868,15 +1894,16 @@ STAGE void build_H(const Ctx c) {
         float acc = 0;
         for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
           const float* cr = SF(con) + i * CON_WORDS;
-          int dim = con_dim(cr);
-          float D = cr[C_D], un = cr[C_U];
+          const int dim = con_dim(cr);
+          const uint32_t act = con_act(cr);
+          float D = cr[C_D];
           float wnr = cr[C_W + r], wns = cr[C_W + s];
-          if (dim == 1) { if (un < 0) acc += D * wnr * wns; continue; }
+          if (dim == 1) { if (act & 1u) acc += D * wnr * wns; continue; }
           float Wnn = 0;
           for (int k = 1; k < dim; k++) {
-            float mu = con_mu(cr, k), uk = cr[C_U + k];
-            float ap = (un + mu * uk) < 0 ? 1.f : 0.f, am = (un - mu * uk) < 0 ? 1.f : 0.f;
+            float ap = (act >> (2 * k - 2)) & 1u ? 1.f : 0.f, am = (act >> (2 * k - 1)) & 1u ? 1.f : 0.f;
             if (ap + am == 0.f) continue;
+            float mu = con_mu(cr, k);
             float wkr, wks;
             if (k < 3) { wkr = cr[C_W + 6 * k + r]; wks = cr[C_W + 6 * k + s]; }
 #ifdef B200_KITCHEN
@@ -2365,18 +2392,14 @@ STAGE LsStep linesearch(const Ctx c, float g1, float g2, float gtol, int maxit) 
 
 #endif
 
-// Newton solver, split so that the iteration loop can be driven block-uniformly (see forward()).
-template <bool HF>
-STAGE void newton_begin(const Ctx c) {
-  ASSUME_SHARED(c);
-  // qacc holds the warm start (previous sub-step's solution); rows become J a - aref = J a + B (J qvel) + K imp r
-  mulM(c, SF(qacc), SF(Ma));
-  rows_begin<HF>(c, SF(qvel), SF(qacc));
-}
+// Newton solver, split so that the iteration loop can be driven block-uniformly (see forward()).  The convergence check ends
+// the stage that brings the solver to its point (newton_begin, newton_move), right after the contact update that parked the
+// base-row forces and the edge activity: no sweep over the contacts, stage call or block barrier of its own.
 
-// forces, gradient and the convergence tests at the current point; returns 1 when the solver is finished
+// gradient and convergence tests at the current point after `iter` moves, the last of which improved the cost by
+// `improvement`; returns 1 when the solver is finished
 template <bool HF>
-STAGE int newton_check(const Ctx c, int iter, float improvement) {
+HD int newton_check(const Ctx c, int iter, float improvement) {
   ASSUME_SHARED(c);
   const DMHead* h = c.h;
   int nv = h->nv;
@@ -2400,6 +2423,19 @@ STAGE int newton_check(const Ctx c, int iter, float improvement) {
   return 0;
 }
 
+// opening of the solve and the check at iteration 0; returns 1 when the warm start is already converged
+template <bool HF>
+STAGE int newton_begin(const Ctx c) {
+  ASSUME_SHARED(c);
+  // qacc holds the warm start (previous sub-step's solution); rows become J a - aref = J a + B (J qvel) + K imp r
+  mulM(c, SF(qacc), SF(Ma));
+  rows_begin<HF>(c, SF(qvel), SF(qacc));
+  CHECK_TIC();
+  const int done = newton_check<HF>(c, 0, 0.f);
+  CHECK_TOC(TM_NBEGIN);
+  return done;
+}
+
 // Newton direction; returns 0 if the direction vanished
 template <int NVP>
 STAGE void newton_direction(const Ctx c) {
@@ -2410,9 +2446,10 @@ STAGE void newton_direction(const Ctx c) {
   spd_solve<NVP>(c, SF(H), nullptr, 0.f, SF(search), SF(H));
 }
 
-// exact line search and move; returns 1 when the solver must stop (no progress possible), *improvement updated
+// exact line search and move number iter, then the check at the new point; returns 0 to go on, 1 when the solver has converged,
+// 2 when it must stop (no progress possible: the point is the one already checked)
 template <bool HF, int LSE>
-STAGE int newton_move(const Ctx c, float* improvement) {
+STAGE int newton_move(const Ctx c, int iter) {
   ASSUME_SHARED(c);
   const DMHead* h = c.h;
   int nv = h->nv;
@@ -2427,23 +2464,31 @@ STAGE int newton_move(const Ctx c, float* improvement) {
   float q1 = 0, q2 = 0, sn = 0;
   LANES(i, nv) { q1 += search[i] * (Ma[i] - fs[i]); q2 += 0.5f * search[i] * Mv[i]; sn += search[i] * search[i]; }
   q1 = wsum(q1); q2 = wsum(q2); sn = sqrtf(wsum(sn));
-  if (sn < 1e-20f) return 1;
+  if (sn < 1e-20f) return 2;
   float gtol = h->tolerance * h->ls_tolerance * sn / scale;
   TOC(TM_MV_ROWS);
   const LsStep ls = linesearch<HF, LSE>(c, q1, q2, gtol, h->ls_iterations < 20 ? h->ls_iterations : 20);
-  *improvement = ls.improve;
   const float alpha = ls.alpha;
   TOC(TM_MV_LS);
-  if (alpha == 0.f) return 1;
+  if (alpha == 0.f) return 2;
   LANES(i, nv) { a[i] += alpha * search[i]; Ma[i] += alpha * Mv[i]; }
-  LANES(i, cnt[CNT_NCON]) { float* cr = SF(con) + i * CON_WORDS; for (int k = 0; k < C_NB; k++) cr[C_U + k] += alpha * cr[C_JV + k]; }
+  LANES(i, cnt[CNT_NCON]) {
+    float* cr = SF(con) + i * CON_WORDS;
+    float U[C_NB];
+#pragma unroll
+    for (int k = 0; k < C_NB; k++) { U[k] = cr[C_U + k] + alpha * cr[C_JV + k]; cr[C_U + k] = U[k]; }
+    contact_park_forces(cr, U);
+  }
   LANES(i, cnt[CNT_NWELD] * 6) { float* wr = SF(weld) + (i / 6) * WELD_WORDS; wr[W_JAR + i % 6] += alpha * wr[W_JV + i % 6]; }
   LANES(i, cnt[CNT_NDR]) { float* dr = SF(dofrow) + i * DR_WORDS; dr[DR_JAR] += alpha * dr[DR_JV]; }
   if (HF) LANES(d, h->nfric) SF(fric)[d] += alpha * SF(fric)[h->nfric + d];
   SYNC();
   if (c.lane == 0) cnt[CNT_ITERS] += 1;
   TOC(TM_MV_UPD);
-  return 0;
+  CHECK_TIC();
+  const int done = newton_check<HF>(c, iter + 1, ls.improve);
+  CHECK_TOC(TM_NMOVE);
+  return done;
 }
 
 // the solve of the implicit-damping Euler step: SF(search) <- (M + h B)^-1 (f_smooth + f_constraint)
@@ -2467,7 +2512,9 @@ HD void forward(const Ctx c, bool active) {
   constexpr bool HF = NVP >= 30;
   constexpr bool CX = NVP == 22 || NVP >= 30;   // NVP 22 = the 21-dof arm build plus the convex collider (FetchSlide)
   constexpr int kLsE = DM_LS_E(NVP);   // line-search edge slots per lane
-  // HF: the hand build (NVP >= 30, 14 warps per block) is faster with a barrier after every stage (DESIGN.md 3, "Hand build")
+  // HF: the hand build (NVP >= 30, 14 warps per block) is faster with a barrier after every stage (DESIGN.md 3, "Hand build").
+  // REBUILD (the 28- and 32-warp kernels): no alignment after the collision stage and between the Newton direction and the move;
+  // with the convergence check inside the move, FetchPickAndPlace at 32 warps runs 1.4 % faster without them (DESIGN.md 6)
   TIC();
   ALIGN(); TOC(TM_BARRIER);
   if (active) kinematics(stage_ctx<REBUILD>(c));
@@ -2475,27 +2522,23 @@ HD void forward(const Ctx c, bool active) {
   if (active) { com_quantities(stage_ctx<REBUILD>(c)); mass_matrix(stage_ctx<REBUILD>(c)); }
   TOC(TM_COM_M); ALIGN(); TOC(TM_BARRIER);
   if (active) collision<HF, CX>(stage_ctx<REBUILD>(c));
-  TOC(TM_COLL); ALIGN(); TOC(TM_BARRIER);
+  TOC(TM_COLL); if (!REBUILD) ALIGN(); TOC(TM_BARRIER);
   if (active) make_constraint<HF>(stage_ctx<REBUILD>(c));
   TOC(TM_CONSTR); if (HF) ALIGN(); TOC(TM_BARRIER);
   if (active) smooth_forces(stage_ctx<REBUILD>(c));
   TOC(TM_SMOOTH); if (HF) ALIGN(); TOC(TM_BARRIER);
-  if (active) newton_begin<HF>(stage_ctx<REBUILD>(c));
+  int done = 1;
+  if (active) done = newton_begin<HF>(stage_ctx<REBUILD>(c));
   TOC(TM_NBEGIN);
-  int done = active ? 0 : 1;
-  float improvement = 0;
   for (int iter = 0;; iter++) {
-    ALIGN(); TOC(TM_BARRIER);
-    if (!done) done = newton_check<HF>(stage_ctx<REBUILD>(c), iter, improvement);
-    TOC(TM_NCHECK);
     bool more = ALIGN_OR(!done);
     TOC(TM_BARRIER);
     if (!more) break;
     if (!done) build_H<HF>(stage_ctx<REBUILD>(c));
     TOC(TM_BUILDH); if (HF) ALIGN(); TOC(TM_BARRIER);
     if (!done) newton_direction<NVP>(stage_ctx<REBUILD>(c));
-    TOC(TM_NDIR); ALIGN(); TOC(TM_BARRIER);
-    if (!done) done = newton_move<HF, kLsE>(stage_ctx<REBUILD>(c), &improvement) ? 2 : 0;
+    TOC(TM_NDIR); if (!REBUILD) ALIGN(); TOC(TM_BARRIER);
+    if (!done) done = newton_move<HF, kLsE>(stage_ctx<REBUILD>(c), iter);
     TOC(TM_NMOVE);
   }
 }
