@@ -142,6 +142,7 @@ struct b200sim {
   unsigned long long* overflow_count = nullptr;  // env-steps that hit a capacity limit (device counter)
   int max_steps = 0, term_on_success = 0;        // b200sim_set_time_limit
   int packed = 0, packed_w = 0;                  // b200sim_set_packed
+  ObsNoiseArgs noise = {nullptr, nullptr, 0, 0};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
   size_t smem_bytes = 0;
   int blocks = 0;
   long launches = 0;
@@ -383,7 +384,7 @@ static int launch(b200sim* h, int mode, int nraw, const float* actions, const un
   io.terminated = terminated; io.truncated = truncated; io.info = info;
   io.elapsed = h->elapsed; io.max_steps = h->max_steps; io.term_on_success = h->term_on_success; io.overflow_count = h->overflow_count;
   ON_DEVICE(h);
-  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io))
+  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io, h->noise))
     return fail(h, "no kernel variant for this (envs per block, nv) pair: nothing was launched", -8);
   h->launches++;
   CUDA_OK(cudaGetLastError());
@@ -395,6 +396,14 @@ int b200sim_step(b200sim_t* h, const float* actions, float* obs, float* achieved
                  unsigned char* terminated, unsigned char* truncated, int* info, void* stream) {
   if (!actions) return fail(h, "b200sim_step: actions is NULL", -1);
   return launch(h, MODE_STEP, 0, actions, nullptr, obs, achieved, desired, reward, success, terminated, truncated, info, stream);
+}
+int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long seed, int env_offset, const int* episode) {
+  if (h->unit != &kernel_unit_kitchen && h->unit != &kernel_unit_kitchen_groups && h->unit != &kernel_unit_kitchen_hull)
+    return fail(h, "b200sim_set_obs_noise: observation noise exists in the kitchen kernel builds only", -6);
+  if (scale && !episode) return fail(h, "b200sim_set_obs_noise: episode is NULL", -1);
+  if (env_offset < 0) return fail(h, "b200sim_set_obs_noise: negative env_offset", -1);
+  h->noise = {scale, scale ? episode : nullptr, seed, env_offset};
+  return 0;
 }
 int b200sim_refresh(b200sim_t* h, const unsigned char* mask, float* obs, float* achieved, float* desired, float* reward,
                     float* success, void* stream) {

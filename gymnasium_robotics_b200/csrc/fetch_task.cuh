@@ -535,29 +535,72 @@ HD void adroit_door_observe(const Ctx& c, const FetchTask& t, float* obs, float*
 }
 
 #ifdef B200_KITCHEN
+#include "reset_sample.cuh"
+// FrankaKitchen observation noise (franka_env.py:114-124, kitchen_env.py:374-385; b200sim_set_obs_noise): block b of the
+// Philox4x32-10 stream (seed; env, episode, step t) holds the uniforms of observation entries 4 b .. 4 b + 3, each in [-1, 1).
+// `t` is the env's step counter after the launch, so that a refresh after set_state(elapsed = t) redraws the noise step t drew.
+// t < 2^28, b < 16; the tag 0x0B5E is used by no other draw (reset_sample.cuh).
+#define RS_OBS_NOISE_TAG 0x0B5Eu
+RS_HD void rs_obs_noise_block(unsigned long long seed, uint32_t env, uint32_t episode, uint32_t t, uint32_t b, float u[4]) {
+  const uint32_t key[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
+  const uint32_t ctr[4] = {env, episode, (t << 4) | b, RS_OBS_NOISE_TAG};
+  uint32_t r[4];
+  rs_philox4x32_10(ctr, key, r);
+  for (int w = 0; w < 4; w++) u[w] = 2.0f * rs_u01(r[w]) - 1.0f;   // exact in fp32: (k - 2^23) / 2^23
+}
+// One env's noise stream in one launch: `scale` holds one amplitude per observation entry, env is the global env index
+struct ObsNoiseKey {
+  const float* scale;
+  unsigned long long seed;
+  uint32_t env, episode, t;
+};
 // FrankaKitchen-v1 (envs/franka_kitchen/franka_env.py:92-128, kitchen_env.py:371-423): the kernel runs do_simulation(ctrl, 40)
-// and returns the noise-free observation robot qpos | robot qvel | object qpos | object qvel (the first nu joints are the
-// robot's) and the full qpos as `achieved`; the position targets (from the last noisy observation), the observation noise
-// and the task bookkeeping are batched host-side tensor code (gymnasium_robotics_b200/kitchen.py), as they are Python in the
-// reference.  [bring-up build]
-HD void kitchen_observe(const Ctx& c, const FetchTask& t, float* obs, float* achieved, float* desired, float* reward, float* success) {
+// and returns the observation robot qpos | robot qvel | object qpos | object qvel (the first nu joints are the robot's) and
+// the full, noise-free qpos as `achieved` (the task bookkeeping reads the true state, kitchen_env.py:356-369).  Without `noise`
+// the observation is noise-free and the host adds the noise (rng_mode "numpy" / "torch"); with it (rng_mode "device") the
+// kernel adds u * scale[j] to entry j, u = uniform j % 4 of block j / 4 of the env's stream, one lane per block.  The
+// position targets and the bookkeeping are batched host-side tensor code (gymnasium_robotics_b200/kitchen.py), as they are
+// Python in the reference.
+HD void kitchen_observe(const Ctx& c, const FetchTask& t, float* obs, float* achieved, float* desired, float* reward, float* success,
+                        const ObsNoiseKey* noise) {
   const DMHead* h = c.h;
   const int nr = h->nu, nq = h->nq, nv = h->nv;
-  LANES(i, nr) { obs[i] = SF(qpos)[i]; obs[nr + i] = SF(qvel)[i]; }
-  LANES(i, nq - nr) obs[2 * nr + i] = SF(qpos)[nr + i];
-  LANES(i, nv - nr) obs[2 * nr + (nq - nr) + i] = SF(qvel)[nr + i];
+  if (noise) {
+    LANES(b, (t.nobs + 3) >> 2) {
+      float u[4];
+      rs_obs_noise_block(noise->seed, noise->env, noise->episode, noise->t, (uint32_t)b, u);
+      for (int w = 0; w < 4; w++) {
+        const int j = 4 * b + w;
+        if (j >= t.nobs) break;
+        const float v = j < nr ? SF(qpos)[j] : (j < 2 * nr ? SF(qvel)[j - nr] : (j < nr + nq ? SF(qpos)[j - nr] : SF(qvel)[j - nq]));
+#ifdef __CUDA_ARCH__
+        obs[j] = v + __fmul_rn(u[w], noise->scale[j]);   // the product rounded on its own, as the host build rounds it
+#else
+        obs[j] = v + u[w] * noise->scale[j];
+#endif
+      }
+    }
+  } else {
+    LANES(i, nr) { obs[i] = SF(qpos)[i]; obs[nr + i] = SF(qvel)[i]; }
+    LANES(i, nq - nr) obs[2 * nr + i] = SF(qpos)[nr + i];
+    LANES(i, nv - nr) obs[2 * nr + (nq - nr) + i] = SF(qvel)[nr + i];
+  }
   LANES(i, nq) { achieved[i] = SF(qpos)[i]; desired[i] = 0.f; }
   if (c.lane == 0) { *reward = 0.f; *success = 0.f; }
-  (void)t;
 }
 #endif
 
 // one env, one warp.  `st` is this env's state record; outputs are this env's rows.  `active` is warp-uniform: idle
 // warps run the same control flow (for the block-wide alignment barriers) but touch no memory.
-// REBUILD: rebuild the context before each stage call (stage_ctx)
+// REBUILD: rebuild the context before each stage call (stage_ctx).  Kitchen builds: `noise`, the env's observation noise (NULL =
+// none); the parameter exists in those builds only, so that the other builds' kernels keep their source and parameters.
 template <int NVP, bool REBUILD = false>
 HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, int nraw, float* st, const float* action, float* obs,
-                       float* achieved, float* desired, float* reward, float* success, int* iters_out) {
+                       float* achieved, float* desired, float* reward, float* success, int* iters_out
+#ifdef B200_KITCHEN
+                       , const ObsNoiseKey* noise = nullptr
+#endif
+                       ) {
   const DMHead* h = c.h;
   if (active) {
     load_state(c, t, st);
@@ -627,7 +670,7 @@ HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, 
     adroit_hammer_observe(c, t, obs, achieved, desired, reward, success);
 #ifdef B200_KITCHEN
   } else if (NVP >= 30 && t.kind == TASK_KITCHEN) {
-    kitchen_observe(c, t, obs, achieved, desired, reward, success);
+    kitchen_observe(c, t, obs, achieved, desired, reward, success, noise);
 #endif
   } else if (NVP >= 30 && t.kind == TASK_ADROIT_DOOR) {
     if (nsub == 0) kinematics(c);

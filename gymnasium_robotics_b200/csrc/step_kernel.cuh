@@ -29,9 +29,23 @@ struct StepIO {
   unsigned long long* overflow_count;      // device counter of env-steps that ran into a capacity limit (NULL = none)
 };
 
+// The observation noise of a handle (b200sim_set_obs_noise): one scale per observation entry (NULL = no noise), the per-env
+// episode counters, the key and the global index of env 0.  A kernel parameter of the kitchen builds only: the other builds' kernels
+// take exactly the parameters they took before it existed.
+struct ObsNoiseArgs {
+  const float* scale; const int* episode; unsigned long long seed; int env_offset;
+};
+#ifdef B200_KITCHEN
+#define B200_KITCHEN_PARAM , ObsNoiseArgs noise_args
+#define B200_KITCHEN_ARG , noise_args
+#else
+#define B200_KITCHEN_PARAM
+#define B200_KITCHEN_ARG
+#endif
+
 template <int WPB, int NVP>
 __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restrict__ model_g, FetchTask task, int mode, int nraw,
-                                                         int N, StepIO io) {
+                                                         int N, StepIO io B200_KITCHEN_PARAM) {
   extern __shared__ __align__(128) uint32_t smem[];
   __shared__ __align__(8) unsigned long long bar;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -74,9 +88,19 @@ __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restr
   const float* act = io.actions ? io.actions + e * task.nact : nullptr;  // only dereferenced in MODE_STEP by active warps
   float* success = io.success + e * io.scalar_stride;
   int iters = 0;
+#ifdef B200_KITCHEN
+  // the noise of the observation this launch returns: the episode that observation belongs to and the step count after the launch
+  // (a step increments `elapsed` below; a refresh -- after a reset, after set_state -- leaves it)
+  const bool noisy = active && noise_args.scale;
+  const ObsNoiseKey noise_key = {noise_args.scale, noise_args.seed, (uint32_t)(noise_args.env_offset + env), noisy ? (uint32_t)noise_args.episode[e] : 0u,
+                                 noisy ? (uint32_t)(io.elapsed[e] + (mode == MODE_STEP ? 1 : 0)) : 0u};
+  fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
+                      io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters, noisy ? &noise_key : nullptr);
+#else
   // (WPB >= 28: at most 72 registers per thread, the driver rebuilds its context before each stage call -- stage_ctx)
   fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
                       io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters);
+#endif
   if (active && lane == 0) {
     // episode bookkeeping of the env-step (TimeLimit wrapper + compute_terminated), flags in both output forms; refresh / raw
     // launches leave the flags of the rows they rewrite alone (a same-step autoreset keeps the flags of the finished episode)
@@ -109,15 +133,15 @@ struct KernelUnit {
   bool (*has)(int wpb, int nvp);                                // an instantiation <wpb, nvp> exists
   cudaError_t (*setattr)(int wpb, int nvp, int smem_bytes);     // cudaErrorInvalidValue when it does not
   bool (*launch)(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev, const FetchTask& task,
-                 int mode, int nraw, int N, const StepIO& io);  // false (nothing launched) when it does not
-};
+                 int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args);  // false (nothing launched) when it does not;
+};                                                                                                  // noise_args reach the kitchen units' kernels only
 
 #define B200_UNIT_HAS(W, V) || (wpb == W && nvp == V)
 #define B200_UNIT_SETATTR(W, V) \
   if (wpb == W && nvp == V) return cudaFuncSetAttribute(fetch_kernel<W, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
 #define B200_UNIT_LAUNCH(W, V)                                                                           \
   if (wpb == W && nvp == V) {                                                                            \
-    fetch_kernel<W, V><<<blocks, W * 32, smem_bytes, stream>>>(model_dev, task, mode, nraw, N, io);      \
+    fetch_kernel<W, V><<<blocks, W * 32, smem_bytes, stream>>>(model_dev, task, mode, nraw, N, io B200_KITCHEN_ARG); \
     return true;                                                                                         \
   }
 
@@ -133,7 +157,7 @@ struct KernelUnit {
     return cudaErrorInvalidValue;                                                                                                    \
   }                                                                                                                                  \
   static bool unit_launch(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev,           \
-                          const FetchTask& task, int mode, int nraw, int N, const StepIO& io) {                                      \
+                          const FetchTask& task, int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args) {      \
     VARIANTS(B200_UNIT_LAUNCH)                                                                                                       \
     return false;                                                                                                                    \
   }                                                                                                                                  \

@@ -183,6 +183,15 @@ class CudaBackend:
         self._check(self.L.b200sim_reset_uniform(self.h, mask.data_ptr() if mask is not None else None, rest_record.data_ptr(), ctypes.byref(params),
                                                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset), episode.data_ptr(), *self._ptrs(out), self._stream()))
 
+    def set_obs_noise(self, scale, seed, env_offset, episode):
+        """b200sim_set_obs_noise (kitchen builds): later launches add u * scale to the observation, u drawn per (seed, env, episode,
+        step); scale None turns the noise off.  The handle keeps both pointers: the tensors must outlive its launches."""
+        if scale is not None:
+            assert scale.is_cuda and scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == self.nobs
+            assert episode.is_cuda and episode.dtype == torch.int32 and episode.is_contiguous() and episode.numel() == self.num_envs
+        self._check(self.L.b200sim_set_obs_noise(self.h, scale.data_ptr() if scale is not None else None, int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                                 int(env_offset), episode.data_ptr() if scale is not None else None))
+
     def reset_maze(self, mask, rest_record, params, goal_xy, reset_xy, seed, env_offset, episode, out):
         """b200sim_reset_maze: goal cell + noise, reset cell away from the goal + noise, then mj_forward + _get_obs."""
         assert rest_record.is_cuda and rest_record.dtype == torch.float32 and rest_record.numel() == self.layout["stride"]

@@ -9,7 +9,7 @@ Mirrors (batched) the reference's Python around the hot path:
       completion / removal / termination bookkeeping -- here as [N, n_tasks] boolean tensors
   * registry: FrankaKitchen-v1, max_episode_steps = 280 (__init__.py:1117-1121)
 The target computation, the noise and the bookkeeping are a few elementwise tensor operations per step (they are Python in
-the reference as well); the 40 sub-steps of physics are one kernel launch.
+the reference as well); the 40 sub-steps of physics are one kernel launch.  With rng_mode="device" the kernel adds the noise itself.
 """
 from __future__ import annotations
 
@@ -63,10 +63,14 @@ class KitchenVectorEnv(VectorEnv):
     """`gym.make_vec("FrankaKitchen-v1", num_envs=N)`.  Observation dict: `observation` [N, 59], `achieved_goal` /
     `desired_goal` dicts task -> [N, k]; reward = number of tasks completed in the step; `terminated` when every task of the
     episode is completed; info carries the bookkeeping as boolean [N, n_tasks] tensors (column order `self.tasks`).
-    The observation is noisy, and the next step's control targets start from it, so there is no `set_state`."""
+    The observation is noisy, and the next step's control targets start from it.  rng_mode="numpy" / "torch" draw the noise on
+    the host and have no `set_state`.  rng_mode="device" draws it in the step kernel (b200sim_set_obs_noise) as a function of
+    (seed, global env index, episode, step), so a run does not depend on batch shape or sharding, and `get_state` / `set_state`
+    checkpoint the env: the record's goal slot, which the kitchen task does not use, carries what the state record lacks --
+    word 0 the episode counter, words 1-2 the seed (int32 bits), then `tasks_to_complete` and `episode_task_completions` (0 / 1)."""
 
     metadata = {"render_modes": [], "render_fps": 12, "autoreset_mode": "next_step"}
-    AUTO_RECOVER = DEVICE_RESET = False
+    AUTO_RECOVER = False
 
     def __init__(self, num_envs: int = 1, tasks_to_complete=None, terminate_on_tasks_completed: bool = True,
                  remove_task_when_completed: bool = True, object_noise_ratio: float = 0.0005, robot_noise_ratio: float = 0.01,
@@ -118,6 +122,10 @@ class KitchenVectorEnv(VectorEnv):
                          backend_factory=make_backend, num_envs=num_envs, device=device, max_episode_steps=max_episode_steps,
                          autoreset_mode=autoreset_mode, rng_mode=rng_mode, n_substeps=frame_skip, kwargs=kwargs)
         self._can_terminate = bool(terminate_on_tasks_completed)
+        if self.rng_mode == "device" and not hasattr(self.backend, "set_obs_noise"):
+            self.backend.close()
+            raise NotImplementedError("rng_mode='device' needs a backend that draws the observation noise in the step "
+                                      f"(set_obs_noise, b200sim_set_obs_noise); {type(self.backend).__name__} has none")
         dev = self.device
         assert int(np.round(1.0 / self.dt)) == self.metadata["render_fps"]      # kitchen_env.py:311-313
         cfg = load_franka_config()                                              # franka_env.py:172-202
@@ -166,7 +174,7 @@ class KitchenVectorEnv(VectorEnv):
 
     def _obs_dict(self, out):
         q = out["achieved"]
-        return self._cast_obs({"observation": self._obs,
+        return self._cast_obs({"observation": out["obs"] if self.rng_mode == "device" else self._obs,
                                "achieved_goal": {t: (q[:, self._run[t]] if self._run[t] is not None else q[:, self._idx[t]]) for t in self.tasks},
                                "desired_goal": {t: self._goal[t].expand(self.num_envs, -1) for t in self.tasks}})
 
@@ -177,8 +185,29 @@ class KitchenVectorEnv(VectorEnv):
         rest[self._sl["qvel"]] = self.init_qvel
         return rest
 
+    def _device_noise(self):
+        """rng_mode="device": the episode counters, the reset without draws and the noise stream of the handle (seed as it stands)."""
+        if self._dev_reset is None:
+            from ._lib import UniformResetC
+
+            p = UniformResetC()
+            p.n, p.quat_slot = 0, -1   # reset_model draws nothing but the observation noise
+            self._dev_reset = p
+            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
+        self.backend.set_obs_noise(self._noise_scale, self._dev_seed, self.env_offset, self._episode)
+        return self._dev_reset
+
     def _reset_envs(self, mask, out, options=None):
         """MujocoEnv.reset -> mj_resetData -> reset_model (franka_env.py:130-137), then KitchenEnv.reset (kitchen_env.py:425-437)."""
+        if self.rng_mode == "device":
+            # record <- rest record, elapsed <- 0, episode += 1, then the refresh draws the noise of (episode, step 0)
+            p = self._device_noise()
+            every = self._reset_all
+            self.backend.reset_uniform(None if every else mask.to(torch.uint8), self._rest, p, self._dev_seed, self.env_offset, self._episode, out)
+            self._todo = self._todo | mask[:, None]
+            self._episode_done = self._episode_done & ~mask[:, None]
+            self._last_robot_qpos = out["obs"][:, :9].clone()
+            return
         idx = self._mask_indices(mask)
         if idx.numel() == 0:
             return
@@ -207,9 +236,12 @@ class KitchenVectorEnv(VectorEnv):
         return self.control_targets(actions)
 
     def _step_results(self, out):
-        # the observation noise of every env is drawn before a NEXT_STEP reset draws its reset noise
-        self._obs = out["obs"] + self._noise(self._all_idx)
-        self._last_robot_qpos = self._obs[:, :9].clone()
+        if self.rng_mode == "device":   # the kernel returned the noisy observation
+            self._last_robot_qpos = out["obs"][:, :9].clone()
+        else:
+            # the observation noise of every env is drawn before a NEXT_STEP reset draws its reset noise
+            self._obs = out["obs"] + self._noise(self._all_idx)
+            self._last_robot_qpos = self._obs[:, :9].clone()
         q = out["achieved"]
         # kitchen_env.py:356-369, 399-423
         # (|| q[task] - goal || < BONUS_THRESH for every task at once; the norm itself, as the reference compares it)
@@ -241,5 +273,35 @@ class KitchenVectorEnv(VectorEnv):
         return sum((torch.linalg.norm(torch.as_tensor(achieved_goal[t]) - torch.as_tensor(desired_goal[t]), dim=-1) < BONUS_THRESH)
                    .to(torch.float32) for t in achieved_goal)
 
+    # ------------------------------------------------------------------ state access (rng_mode="device")
+    def get_state(self):
+        state, elapsed = super().get_state()
+        if self.rng_mode == "device":
+            self._device_noise()
+            g, k = self.backend.layout["goal"], len(self.tasks)
+            state[:, g].view(torch.int32).copy_(self._episode)
+            seed = self._dev_seed & 0xFFFFFFFFFFFFFFFF
+            words = torch.tensor([seed & 0xFFFFFFFF, seed >> 32], dtype=torch.int64).to(torch.int32)   # two's-complement wrap
+            state[:, g + 1:g + 3].view(torch.int32).copy_(words.to(self.device).expand(self.num_envs, 2))
+            state[:, g + 3:g + 3 + k] = self._todo.to(torch.float32)
+            state[:, g + 3 + k:g + 3 + 2 * k] = self._episode_done.to(torch.float32)
+        return state, elapsed
+
     def set_state(self, state, elapsed=None):
-        raise NotImplementedError("FrankaKitchen has no set_state: its noisy observation and last robot pose are not part of the record")
+        """rng_mode="device" only: a record of `get_state` (with its bookkeeping) and the step counters; the refresh redraws the
+        noise of (seed, env, episode, step), so the observation and the next control targets are those of the saved env."""
+        if self.rng_mode != "device":
+            raise NotImplementedError("FrankaKitchen has set_state in rng_mode='device' only: with host-drawn noise the noisy observation "
+                                      "and the last robot pose are not part of the record")
+        state = torch.as_tensor(state).to(self.device, torch.float32)
+        g, k = self.backend.layout["goal"], len(self.tasks)
+        words = state[:, g:g + 3].contiguous().view(torch.int32)
+        lo, hi = (int(w) & 0xFFFFFFFF for w in words[0, 1:3].tolist())
+        self._dev_seed = lo | (hi << 32)
+        self._device_noise()
+        self._episode.copy_(words[:, 0])
+        self._todo = state[:, g + 3:g + 3 + k] != 0
+        self._episode_done = state[:, g + 3 + k:g + 3 + 2 * k] != 0
+        obs = super().set_state(state, elapsed)
+        self._last_robot_qpos = self._last["obs"][:, :9].clone()
+        return obs

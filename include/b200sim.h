@@ -151,6 +151,14 @@ typedef struct b200sim_uniform_reset {
 int b200sim_reset_uniform(b200sim_t* h, const unsigned char* mask, const float* rest_record, const b200sim_uniform_reset_t* params,
                           unsigned long long seed, int env_offset, int* episode, float* obs, float* achieved, float* desired,
                           float* reward, float* success, void* stream);
+/* Observation noise drawn in the step kernel (FrankaKitchen, reference: franka_env.py:114-124, kitchen_env.py:374-385; kitchen
+ * kernel builds only, any other handle returns an error).  From the next launch on, every step, refresh and reset adds
+ * u * scale[j] to observation entry j, u uniform in [-1, 1) from Philox4x32-10 keyed by `seed`, counter (env index + env_offset,
+ * episode[i], (t << 4) | j / 4, 0x0B5E), word j % 4; t is the env's step counter after the launch (b200sim_elapsed: + 1 for a
+ * step, unchanged for a refresh, 0 after a reset).  `scale` (device, [nobs] floats) and `episode` (device, [N] int32: the counters
+ * that b200sim_reset_uniform increments) are read by every later launch and must outlive them.  scale NULL: noise off.  The
+ * `achieved` columns (qpos) stay noise-free.  A reset is b200sim_reset_uniform with n = 0 draws. */
+int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long seed, int env_offset, const int* episode);
 /* Maze family (AntMaze / PointMaze; reference: envs/maze/maze_v4.py:256-297, 299-373): goal cell + noise, reset cell farther than
  * half a cell from the goal + noise.  goal_xy / reset_xy: DEVICE tables [n_goal, 2] / [n_reset, 2] of cell centres
  * (MazeEnv.maze.unique_goal_locations / unique_reset_locations, or all free cells when the map marks none, maze_v4.py:212-228). */
