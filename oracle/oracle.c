@@ -1815,6 +1815,13 @@ ACC(qfrc_constraint, qfrc_constraint) ACC(efc_J, J) ACC(efc_force, efc_force) AC
 ACC(efc_pos, efc_pos) ACC(efc_D, efc_D) ACC(efc_R, efc_R) ACC(sensordata, sensordata) ACC(subtree_com, subtree_com)
 ACC(cdof, cdof) ACC(qfrc_actuator, qfrc_actuator) ACC(qfrc_passive, qfrc_passive)
 real* oracle_time(oracle_sim* s) { return &s->time; }
+/* per constraint row: type (ROW_*), object (equality, dof, joint or njnt + tendon, contact), and K, B, imp, impP of aref */
+int* oracle_efc_type(oracle_sim* s) { return s->efc_type; }
+int* oracle_efc_id(oracle_sim* s) { return s->efc_id; }
+real* oracle_efc_KBIP(oracle_sim* s) { return &s->efc_KBIP[0][0]; }
+real* oracle_efc_margin(oracle_sim* s) { return s->efc_margin; }
+/* translational and rotational Jacobian (3 x nv each) of a point fixed to a body, at the current kinematics */
+void oracle_jac_point(const oracle_sim* s, int body, const real* point, real* jacp, real* jacr) { jac_point(s, body, point, jacp, jacr); }
 int oracle_ncon(const oracle_sim* s) { return s->ncon; }
 int oracle_nefc(const oracle_sim* s) { return s->nefc; }
 int oracle_solver_iter(const oracle_sim* s) { return s->solver_iter; }

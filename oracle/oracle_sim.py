@@ -67,6 +67,8 @@ def lib():
         L.oracle_step.restype = None
         L.oracle_jac_site.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]
         L.oracle_contact.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+        L.oracle_jac_point.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+        L.oracle_jac_point.restype = None
         for f in ("oracle_ncon", "oracle_nefc", "oracle_solver_iter", "oracle_overflow"):
             getattr(L, f).argtypes = [ctypes.c_void_p]
             getattr(L, f).restype = ctypes.c_int
@@ -191,10 +193,25 @@ class OracleSim:
                             geom1=int(buf[14]), geom2=int(buf[15]), efc_address=int(buf[16]), pair=int(buf[17])))
         return out
 
+    # efc_type values (oracle.c ROW_*)
+    ROW_EQ, ROW_FRICTION, ROW_LIMIT, ROW_CONTACT = 0, 1, 2, 3
+
     def efc(self, name):
+        """A copy of a constraint-row array: J (nefc x nv), KBIP (nefc x 4: K, B, imp, impP of aref), type and id (int), or a
+        per-row scalar (pos, margin, D, R, aref, force)."""
         fn = getattr(self._L, "oracle_efc_" + name)
-        fn.restype = ctypes.POINTER(ctypes.c_double)
+        integer = name in ("type", "id")
+        fn.restype = ctypes.POINTER(ctypes.c_int if integer else ctypes.c_double)
         fn.argtypes = [ctypes.c_void_p]
-        n = self.nefc * (self.model.nv if name == "J" else 1)
+        w = {"J": self.model.nv, "KBIP": 4}.get(name, 1)
+        n = self.nefc * w
         a = np.ctypeslib.as_array(fn(self._h), shape=(max(n, 1),))[:n].copy()
-        return a.reshape(self.nefc, -1) if name == "J" else a
+        return a.reshape(self.nefc, w) if w > 1 else a
+
+    def jac_point(self, body, point):
+        """(jacp, jacr), 3 x nv each: the Jacobian of a point fixed to `body`, at the current kinematics."""
+        nv = self.model.nv
+        jp, jr = np.zeros((3, nv)), np.zeros((3, nv))
+        pt = np.ascontiguousarray(point, dtype=np.float64)
+        self._L.oracle_jac_point(self._h, int(body), pt.ctypes.data, jp.ctypes.data, jr.ctypes.data)
+        return jp, jr

@@ -88,7 +88,7 @@ def spd(nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
         raise RuntimeError(f"devsim_spd(nvp={nvp}): {L.devsim_last_error().decode()}")
 
 
-STAGE_COLLIDE, STAGE_KIN = 0, 1
+STAGE_COLLIDE, STAGE_KIN, STAGE_PROBLEM, STAGE_JV, STAGE_BUILD_H = 0, 1, 2, 3, 4
 LAYOUT = ("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE")
 
 
@@ -96,7 +96,7 @@ class DevModel:
     """The device model of `model` as the `flavor` unit builds it, and single stages of that unit on batches of scratch images."""
 
     def __init__(self, flavor, model, eq_data=None, ref=(1.0, 0.75, 0.4), penv_body=-1, ngrp_cap=0):
-        self.flavor, self.model = flavor, model
+        self.flavor, self.model, self.ref = flavor, model, np.asarray(ref, np.float32).astype(np.float64)
         L = self._L = lib(flavor)
         blob = model.to_blob()
         eq = np.ascontiguousarray(eq_data, dtype=np.float64) if eq_data is not None else None
@@ -127,7 +127,7 @@ class DevModel:
         return o
 
     def run(self, nvp, stage, scratch):
-        """stage (STAGE_COLLIDE / STAGE_KIN) of the NVP = nvp instantiation on scratch images [n, scr_words] float32, in place."""
+        """stage (STAGE_COLLIDE / STAGE_KIN / STAGE_PROBLEM / STAGE_JV / STAGE_BUILD_H) of the NVP = nvp instantiation on scratch images [n, scr_words] float32, in place."""
         assert scratch.dtype == np.float32 and scratch.flags.c_contiguous and scratch.shape[1] == self.scr_words
         rc = self._L.devsim_stage(self._h, int(nvp), int(stage), scratch.shape[0], scratch.ctypes.data)
         if rc != 0:

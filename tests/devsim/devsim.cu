@@ -15,6 +15,11 @@
 // them -- read from the global model, one env's scratch after the hot words.  The host hands in a whole scratch image per case
 // and gets the whole image back.  collide = collision<HF, CX> with HF and CX derived from NVP as forward<NVP> derives them;
 // kin = kinematics, com_quantities and mass_matrix.
+//
+// problem / jv: the problem the Newton solver is given.  problem = every stage forward<NVP> runs up to the first direction solve:
+// kinematics, com_quantities, mass_matrix, collision<HF, CX>, make_constraint<HF>, smooth_forces, newton_begin<HF> (M qacc of the
+// warm start, rows_begin, the check: fcon through pass_F and grad) and build_H<HF>.  jv = rows_from_vec<HF>(c, SF(search)) on an image
+// that problem returned: with a unit vector in search it reads one column of the kernel's implicit J into the rows' JV slots.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -118,7 +123,7 @@ done:
   return rc;
 }
 
-enum { DEVSIM_COLLIDE = 0, DEVSIM_KIN = 1 };
+enum { DEVSIM_COLLIDE = 0, DEVSIM_KIN = 1, DEVSIM_PROBLEM = 2, DEVSIM_JV = 3, DEVSIM_BUILD_H = 4 };
 
 template <int NVP>
 __global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ model, int stage, float* scratch) {
@@ -137,7 +142,16 @@ __global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ 
   constexpr bool HF = NVP >= 30;
   constexpr bool CX = NVP == 22 || NVP >= 30;
   if (stage == DEVSIM_COLLIDE) collision<HF, CX>(c);
-  else { kinematics(c); com_quantities(c); mass_matrix(c); }
+  else if (stage == DEVSIM_KIN) { kinematics(c); com_quantities(c); mass_matrix(c); }
+  else if (stage == DEVSIM_PROBLEM) {
+    kinematics(c); com_quantities(c); mass_matrix(c);
+    collision<HF, CX>(c);
+    make_constraint<HF>(c);
+    smooth_forces(c);
+    newton_begin<HF>(c);
+    build_H<HF>(c);
+  } else if (stage == DEVSIM_JV) rows_from_vec<HF>(c, SF(search));
+  else build_H<HF>(c);
   __syncwarp();
   for (int k = lane; k < sw; k += 32) scratch[(size_t)e * sw + k] = s[k];
 }
@@ -192,7 +206,7 @@ int devsim_offset(void* p, const char* name, int model_array) {
   return -1;
 }
 
-// run one stage (DEVSIM_COLLIDE, DEVSIM_KIN) of the NVP = nvp instantiation on ncase scratch images [ncase][scr_words], one block
+// run one stage (DEVSIM_COLLIDE, DEVSIM_KIN, DEVSIM_PROBLEM, DEVSIM_JV, DEVSIM_BUILD_H) of the NVP = nvp instantiation on ncase scratch images [ncase][scr_words], one block
 // each; the images are overwritten with the scratch after the stage.  Returns 0, -1 for an NVP this library does not instantiate,
 // -2 on a CUDA error.
 int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch) {

@@ -89,8 +89,9 @@ def lib(wide=False):
         L.hostsim_env_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 7
         L.hostsim_spd.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
         L.hostsim_spd.restype = ctypes.c_int
-        L.hostsim_collide.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.hostsim_collide.restype = None
+        for f in ("hostsim_collide", "hostsim_problem", "hostsim_jv", "hostsim_build_h"):
+            getattr(L, f).argtypes = [ctypes.c_void_p, ctypes.c_int]
+            getattr(L, f).restype = None
         L.hostsim_model_offset.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
         L.hostsim_model.restype = ctypes.POINTER(ctypes.c_uint32)
         L.hostsim_model.argtypes = [ctypes.c_void_p]
@@ -163,6 +164,18 @@ class HostSim:
     def collide(self, nvp):
         """The collision stage alone, compiled as forward<nvp> compiles it (HF, CX)."""
         self._L.hostsim_collide(self._h, int(nvp))
+
+    def problem(self, nvp):
+        """Every stage forward<nvp> runs up to the first direction solve (tests/devsim STAGE_PROBLEM)."""
+        self._L.hostsim_problem(self._h, int(nvp))
+
+    def jv(self, nvp):
+        """The rows' JV slots <- J search, rows_from_vec<HF> (tests/devsim STAGE_JV)."""
+        self._L.hostsim_jv(self._h, int(nvp))
+
+    def build_h(self, nvp):
+        """build_H<HF> alone (tests/devsim STAGE_BUILD_H)."""
+        self._L.hostsim_build_h(self._h, int(nvp))
 
     def offset(self, name):
         o = self._L.hostsim_offset(self._h, name.encode())

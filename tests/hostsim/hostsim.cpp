@@ -58,6 +58,17 @@ struct HostSim {
   std::string err;
 };
 
+// the problem the Newton solver is given, as tests/devsim's problem op runs it: every stage forward<nvp> runs up to the first
+// direction solve (kinematics ... newton_begin, build_H), with HF and CX derived from nvp
+template <bool HF, bool CX> static void problem_stages(const Ctx& c) {
+  kinematics(c); com_quantities(c); mass_matrix(c);
+  collision<HF, CX>(c);
+  make_constraint<HF>(c);
+  smooth_forces(c);
+  newton_begin<HF>(c);
+  build_H<HF>(c);
+}
+
 extern "C" {
 void* hostsim_create(const void* blob, size_t n, const double* eq_data, const float* ref, int penv_body, int ngrp_cap) {
   HostSim* s = new HostSim;
@@ -97,6 +108,25 @@ void hostsim_collide(void* p, int nvp) {
   if (hf) warp_call(base, [](const Ctx& c) { collision<true, true>(c); });
   else if (cx) warp_call(base, [](const Ctx& c) { collision<false, true>(c); });
   else warp_call(base, [](const Ctx& c) { collision<false, false>(c); });
+}
+void hostsim_problem(void* p, int nvp) {
+  const Ctx& base = ((HostSim*)p)->ctx;
+  const bool hf = nvp >= 30, cx = nvp == 22 || nvp >= 30;
+  if (hf) warp_call(base, [](const Ctx& c) { problem_stages<true, true>(c); });
+  else if (cx) warp_call(base, [](const Ctx& c) { problem_stages<false, true>(c); });
+  else warp_call(base, [](const Ctx& c) { problem_stages<false, false>(c); });
+}
+// the rows' JV slots <- J search (rows_from_vec<HF>) on a scratch that hostsim_problem left
+void hostsim_jv(void* p, int nvp) {
+  const Ctx& base = ((HostSim*)p)->ctx;
+  if (nvp >= 30) warp_call(base, [](const Ctx& c) { rows_from_vec<true>(c, SF(search)); });
+  else warp_call(base, [](const Ctx& c) { rows_from_vec<false>(c, SF(search)); });
+}
+// build_H<HF> alone, on a scratch that hostsim_problem left
+void hostsim_build_h(void* p, int nvp) {
+  const Ctx& base = ((HostSim*)p)->ctx;
+  if (nvp >= 30) warp_call(base, [](const Ctx& c) { build_H<true>(c); });
+  else warp_call(base, [](const Ctx& c) { build_H<false>(c); });
 }
 int hostsim_model_offset(void* p, const char* name) {
   const DMHead* h = ((HostSim*)p)->ctx.h;
