@@ -78,6 +78,29 @@ __global__ void maze_reset_kernel(b200sim_maze_reset_t p, const float* __restric
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
 
+// b200sim_set_goal_update: after a step, one thread per env redraws the goal of an env whose achieved position (qpos[0:2], as the
+// step kernel left it) lies within the success radius; the others are only read
+struct GoalUpdateArgs {
+  const float* goal_xy;   // NULL: update off
+  int n_goal;
+  float scaling, noise;
+  unsigned long long seed;
+  int env_offset;
+  const int* episode;
+};
+__global__ void maze_goal_update_kernel(GoalUpdateArgs g, float radius, int N, int stride, int st_qpos, int st_goal, float* __restrict__ state,
+                                        const int* __restrict__ elapsed) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  float* rec = state + (size_t)i * stride;
+  const float ach[2] = {rec[st_qpos], rec[st_qpos + 1]};
+  float goal[2] = {rec[st_goal], rec[st_goal + 1]};
+  if (rs_maze_goal_update(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
+                          (uint32_t)elapsed[i], ach, goal)) {
+    rec[st_goal] = goal[0]; rec[st_goal + 1] = goal[1];
+  }
+}
+
 __global__ void check_state_kernel(int N, int stride, float* __restrict__ state, const float* __restrict__ rest, b200sim_keep_t keep,
                                    unsigned char* __restrict__ bad) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -143,6 +166,7 @@ struct b200sim {
   int max_steps = 0, term_on_success = 0;        // b200sim_set_time_limit
   int packed = 0, packed_w = 0;                  // b200sim_set_packed
   ObsNoiseArgs noise = {nullptr, nullptr, 0, 0};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
+  GoalUpdateArgs goal_update = {nullptr, 0, 0.f, 0.f, 0, 0, nullptr};   // b200sim_set_goal_update (maze tasks)
   size_t smem_bytes = 0;
   int blocks = 0;
   long launches = 0;
@@ -395,7 +419,23 @@ static int launch(b200sim* h, int mode, int nraw, const float* actions, const un
 int b200sim_step(b200sim_t* h, const float* actions, float* obs, float* achieved, float* desired, float* reward, float* success,
                  unsigned char* terminated, unsigned char* truncated, int* info, void* stream) {
   if (!actions) return fail(h, "b200sim_step: actions is NULL", -1);
-  return launch(h, MODE_STEP, 0, actions, nullptr, obs, achieved, desired, reward, success, terminated, truncated, info, stream);
+  const int rc = launch(h, MODE_STEP, 0, actions, nullptr, obs, achieved, desired, reward, success, terminated, truncated, info, stream);
+  if (rc != 0 || !h->goal_update.goal_xy) return rc;
+  ON_DEVICE(h);
+  maze_goal_update_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->task.success_radius, h->N, h->task.st_stride,
+                                                                               h->task.st_qpos, h->task.st_goal, h->state, h->elapsed);
+  h->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
+                            int env_offset, const int* episode) {
+  if (h->task.kind != TASK_ANTMAZE) return fail(h, "b200sim_set_goal_update: not a maze task", -6);
+  if (goal_xy && !episode) return fail(h, "b200sim_set_goal_update: episode is NULL", -1);
+  if (goal_xy && n_goal < 2) return fail(h, "b200sim_set_goal_update: fewer than two goal cells", -1);
+  if (env_offset < 0) return fail(h, "b200sim_set_goal_update: negative env_offset", -1);
+  h->goal_update = goal_xy ? GoalUpdateArgs{goal_xy, n_goal, scaling, noise, seed, env_offset, episode} : GoalUpdateArgs{nullptr, 0, 0.f, 0.f, 0, 0, nullptr};
+  return 0;
 }
 int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long seed, int env_offset, const int* episode) {
   if (h->unit != &kernel_unit_kitchen && h->unit != &kernel_unit_kitchen_groups && h->unit != &kernel_unit_kitchen_hull)

@@ -142,6 +142,51 @@ RS_HD void rs_maze_reset_draw(const b200sim_maze_reset_t& p, const float* goal_x
   pos[1] += (2.0f * rs_u01(r[1]) - 1.0f) * amp;
 }
 
+// Goal update of a continuing maze task (envs/maze/maze_v4.py:400-418 update_goal, called at the end of every step when
+// reset_target=True): while the achieved position `ach` lies within `radius` of the goal, the goal becomes a new goal cell + noise.
+// The distance is antmaze_observe's (csrc/fetch_task.cuh), rounding for rounding, so the update fires exactly when the step's
+// success column is 1.  Candidate c comes from one Philox block at counter (env, episode, step, RS_MAZE_GOAL_TAG | c << 16), step
+// being the env's step counter after the step: word 0 picks the cell as in rs_maze_reset_draw, words 1 and 2 the noise.  Each
+// product and sum of a candidate is rounded on its own (no FMA contraction), so a restatement in fp32 gives the same bits.
+// Returns the number of candidates drawn, 0 when the goal stays.
+#define RS_MAZE_GOAL_TAG 0x60A1u
+// 64 candidates at most; when all are rejected the goal is the last one.  A candidate is rejected when it lands within 0.45 of `ach`:
+// the noise boxes (side 0.5 x scaling) of the goal cells are disjoint, and a disc of radius 0.45 covers at most one box's worth of
+// them at scaling 1 (PointMaze) and 0.16 of one box at scaling 4 (AntMaze), so with n >= 2 goal cells one candidate is rejected
+// with probability <= 1/2 resp. 0.08, and all 64 with probability <= 5e-20 resp. 5e-71
+#define RS_MAZE_GOAL_CANDIDATES 64
+RS_HD float rs_maze_goal_distance(const float ach[2], const float goal[2]) {
+  float dx = ach[0] - goal[0], dy = ach[1] - goal[1];
+#ifdef __CUDA_ARCH__
+  return sqrtf(fmaf(dy, dy, __fmul_rn(dx, dx)));
+#else
+  return sqrtf(dx * dx + dy * dy);
+#endif
+}
+RS_HD int rs_maze_goal_update(const float* goal_xy, int n_goal, float scaling, float noise, float radius, unsigned long long seed,
+                              uint32_t env, uint32_t episode, uint32_t step, const float ach[2], float goal[2]) {
+  if (!(rs_maze_goal_distance(ach, goal) <= radius)) return 0;
+  const uint32_t key[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
+  const float amp = noise * scaling;
+  int c = 0;
+  while (c < RS_MAZE_GOAL_CANDIDATES) {
+    uint32_t ctr[4] = {env, episode, step, RS_MAZE_GOAL_TAG | ((uint32_t)c << 16)}, r[4];
+    rs_philox4x32_10(ctr, key, r);
+    c++;
+    uint32_t gi = (uint32_t)(((uint64_t)r[0] * (uint64_t)n_goal) >> 32);
+    const float nx = 2.0f * rs_u01(r[1]) - 1.0f, ny = 2.0f * rs_u01(r[2]) - 1.0f;   // exact
+#ifdef __CUDA_ARCH__
+    goal[0] = __fadd_rn(goal_xy[2 * gi], __fmul_rn(nx, amp));
+    goal[1] = __fadd_rn(goal_xy[2 * gi + 1], __fmul_rn(ny, amp));
+#else
+    goal[0] = goal_xy[2 * gi] + nx * amp;
+    goal[1] = goal_xy[2 * gi + 1] + ny * amp;
+#endif
+    if (!(rs_maze_goal_distance(ach, goal) <= radius)) break;
+  }
+  return c;
+}
+
 RS_HD void rs_maze_reset_record(const b200sim_maze_reset_t& p, const float* goal_xy, const float* reset_xy, unsigned long long seed, uint32_t env,
                                 uint32_t episode, const float* rest, int stride, int st_qpos, int st_goal, float* rec) {
   float goal[2], pos[2];

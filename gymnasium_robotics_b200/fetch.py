@@ -192,6 +192,17 @@ class CudaBackend:
         self._check(self.L.b200sim_set_obs_noise(self.h, scale.data_ptr() if scale is not None else None, int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                  int(env_offset), episode.data_ptr() if scale is not None else None))
 
+    def set_goal_update(self, goal_xy, scaling, noise, seed, env_offset, episode):
+        """b200sim_set_goal_update (maze tasks): every later step redraws the goal of the envs that succeeded, per (seed, env,
+        episode, step); goal_xy None turns the update off.  The handle keeps both pointers: the tensors must outlive its steps."""
+        if goal_xy is not None:
+            assert goal_xy.is_cuda and goal_xy.dtype == torch.float32 and goal_xy.is_contiguous() and goal_xy.dim() == 2 and goal_xy.shape[1] == 2
+            assert episode.is_cuda and episode.dtype == torch.int32 and episode.is_contiguous() and episode.numel() == self.num_envs
+        on = goal_xy is not None
+        self._check(self.L.b200sim_set_goal_update(self.h, goal_xy.data_ptr() if on else None, len(goal_xy) if on else 0, float(scaling),
+                                                   float(noise), int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset),
+                                                   episode.data_ptr() if on else None))
+
     def reset_maze(self, mask, rest_record, params, goal_xy, reset_xy, seed, env_offset, episode, out):
         """b200sim_reset_maze: goal cell + noise, reset cell away from the goal + noise, then mj_forward + _get_obs."""
         assert rest_record.is_cuda and rest_record.dtype == torch.float32 and rest_record.numel() == self.layout["stride"]

@@ -148,7 +148,8 @@ class MazeVectorEnv(VectorEnv):
     `model`.  `maze_map=` is the reference's custom layout (point_maze.py:195-207, ant_maze_v5.py:221-229): a list of rows of
     0, 1, "r", "g", "c" cells (`check_maze_map`), built on the agent's committed model (`models.build_maze_model`) unless a
     `model` is given; the named `maze` still supplies the episode length.  The per-env numpy streams exist in every rng_mode:
-    explicit `options` cells and the goal update of `reset_target` draw from them."""
+    explicit `options` cells draw from them, and so does the goal update of `reset_target` except in rng_mode="device", where
+    the step launch redraws the goals of the envs that succeeded (b200sim_set_goal_update)."""
 
     metadata = {"render_modes": [], "render_fps": 50, "autoreset_mode": "next_step"}
     AGENT = "ant"
@@ -203,6 +204,12 @@ class MazeVectorEnv(VectorEnv):
         self.init_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)
         self._goal_loc = torch.as_tensor(self.cells.goal_locations, dtype=torch.float32, device=self.device)
         self._reset_loc = torch.as_tensor(self.cells.reset_locations, dtype=torch.float32, device=self.device)
+        # update_goal (maze_v4.py:400-418) acts only in a continuing task with reset_target and more than one goal location; in
+        # rng_mode="device" the step launch does it (b200sim_set_goal_update), keyed by the seed the library was last given
+        self._goal_update_on = continuing_task and reset_target and len(self.cells.goal_locations) > 1
+        self._goal_update_seed = None
+        if self.rng_mode == "device" and self._goal_update_on and not hasattr(self.backend, "set_goal_update"):
+            raise NotImplementedError(f"{type(self.backend).__name__} cannot update goals on the device (no set_goal_update)")
 
     # ------------------------------------------------------------------ sampling (MazeEnv.reset, maze_v4.py:299-358)
     def _noise_np(self, rng, xy):
@@ -251,7 +258,7 @@ class MazeVectorEnv(VectorEnv):
         rest[self._sl["qpos"]] = self.init_qpos
         return rest
 
-    def _device_reset(self, mask, out):
+    def _device_tables(self):
         if self._dev_reset is None:
             from ._lib import MazeResetC
 
@@ -259,13 +266,23 @@ class MazeVectorEnv(VectorEnv):
             p.n_goal, p.n_reset, p.scaling, p.noise = len(self._goal_loc), len(self._reset_loc), float(self.scaling), float(NOISE)
             self._dev_reset = (p, self._rest, self._goal_loc.contiguous(), self._reset_loc.contiguous())
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
-        p, rest, gl, rl = self._dev_reset
+        if self._goal_update_on and self._goal_update_seed != self._dev_seed:   # first reset, or reset(seed=...) gave a new key
+            self.backend.set_goal_update(self._dev_reset[2], self.scaling, NOISE, self._dev_seed, self.env_offset, self._episode)
+            self._goal_update_seed = self._dev_seed
+        return self._dev_reset
+
+    def _device_reset(self, mask, out):
+        p, rest, gl, rl = self._device_tables()
         self.backend.reset_maze(mask.to(torch.uint8), rest, p, gl, rl, self._dev_seed, self.env_offset, self._episode, out)
         self._elapsed.masked_fill_(mask, 0)
 
     def _reset_envs(self, mask, out, options=None):
-        if self.rng_mode == "device" and not options:   # explicit cells keep the reference-ordered host path
-            return self._device_reset(mask, out)
+        if self.rng_mode == "device":
+            if not options:   # explicit cells keep the reference-ordered host path
+                return self._device_reset(mask, out)
+            # ... and start a new episode of the device streams too, so that the next goal updates draw fresh numbers
+            self._device_tables()
+            self._episode += mask.to(torch.int32)
         idx = self._mask_indices(mask)
         if idx.numel() == 0:
             return
@@ -295,23 +312,28 @@ class MazeVectorEnv(VectorEnv):
         return super()._mask_results(out, pre, reward, terminated, truncated, info)
 
     def _after_autoreset(self, out, info):
-        success = info["success"]
-        if self.continuing_task and self.reset_target and len(self.cells.goal_locations) > 1 and bool(success.any()):
-            self._update_goal(success, out)  # maze_v4.py:400-418 (never for the envs that were just reset: `success` is masked)
+        # rng_mode="device": the step launch has updated the goals already (the envs it reset got the reset draw after it)
+        if self._goal_update_on and self.rng_mode != "device":
+            self._update_goal(info["success"], out)  # maze_v4.py:400-418 (never for the envs that were just reset: `success` is masked)
 
     def _finish_info(self, out, info):
         pass   # `success` as of the step, before a SAME_STEP reset; no mask entry
 
     def _update_goal(self, success, out):
+        """update_goal on the host, from each succeeding env's numpy stream in the reference's order: one read of their achieved
+        goals and goals, one write of the new goals."""
         idx = torch.nonzero(success, as_tuple=False).flatten()
+        if idx.numel() == 0:
+            return
         st, sl = self.backend.state, self._sl
-        for i in idx.tolist():
-            ag = out["achieved"][i].double().cpu().numpy()
-            goal = st[i, sl["goal"]].double().cpu().numpy()
-            rng = self._np_rngs[i]
+        cur = torch.cat([out["achieved"][idx], st[idx, sl["goal"]]], dim=1).double().cpu().numpy()
+        new = cur[:, 2:].copy()
+        for k, i in enumerate(idx.tolist()):
+            ag, goal, rng = cur[k, :2], new[k], self._np_rngs[i]
             while np.linalg.norm(ag - goal) <= SUCCESS_RADIUS:
                 goal = self._noise_np(rng, self.cells.goal_locations[rng.integers(low=0, high=len(self.cells.goal_locations))].copy())
-            st[i, sl["goal"]] = torch.as_tensor(goal, dtype=torch.float32, device=self.device)
+            new[k] = goal
+        st[idx, sl["goal"].start:sl["goal"].stop] = torch.as_tensor(new, dtype=torch.float32, device=self.device)
 
     def _reward_np_dtype(self):
         return np.float64

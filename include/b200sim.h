@@ -169,6 +169,17 @@ typedef struct b200sim_maze_reset {
 int b200sim_reset_maze(b200sim_t* h, const unsigned char* mask, const float* rest_record, const b200sim_maze_reset_t* params,
                        const float* goal_xy, const float* reset_xy, unsigned long long seed, int env_offset, int* episode, float* obs,
                        float* achieved, float* desired, float* reward, float* success, void* stream);
+/* Goal update of a continuing maze task (reference: maze_v4.py:400-418 update_goal, reset_target=True; maze tasks only, any other
+ * handle returns an error).  From the next b200sim_step on, a small kernel runs after the step kernel on the same stream: an env
+ * whose achieved position lies within the task's success_radius of its goal (exactly the envs whose success column is 1) gets a
+ * new goal, redrawn as a goal cell of `goal_xy` (DEVICE table [n_goal, 2]) + noise * scaling * U(-1, 1) per axis until it lies
+ * farther than success_radius, 64 candidates at most.  The draws are Philox4x32-10 keyed by `seed`, counter (env index +
+ * env_offset, episode[i], the env's step counter after the step, 0x60A1 | candidate << 16).  The step's outputs carry the old
+ * goal, as the reference's observation does.  `goal_xy` and `episode` (device, [N] int32: the counters that b200sim_reset_maze
+ * increments) are read by every later step and must outlive them.  goal_xy NULL: update off.  b200sim_raw_step*,
+ * b200sim_refresh and the resets never update the goal. */
+int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
+                            int env_offset, const int* episode);
 /* Shadow-Hand manipulation (reference: envs/shadow_dexterous_hand/manipulate.py:154-224 _reset_sim, :226-279 _sample_goal).  The
  * reference's reset is a retry loop, so the draws are two calls: `b200sim_reset_hand_pose` writes rest_record + the drawn object
  * start pose into the masked envs' records (their goal survives) for attempt number `attempt` -- the caller then settles with
