@@ -72,6 +72,8 @@ def make_vec(env_id: str, num_envs: int = 1, **kwargs):
         raise KeyError(f"{env_id!r} is not provided by the CUDA path yet; available: {sorted(ENV_IDS)}")
     spec = dict(ENV_IDS[env_id])
     spec.update(kwargs)
+    if env_id.startswith("AntMaze_"):
+        spec["ant_version"] = int(env_id[-1])   # the Ant the id wraps: Ant-v5 (-v5) or Ant-v4 (-v4)
     if "maze" in spec:
         from .maze import MazeVectorEnv
 
@@ -115,5 +117,7 @@ def register_envs():
             kw["task"] = kw.pop("hand_task")
         if "adroit_task" in kw:
             kw["task"] = kw.pop("adroit_task")
+        if env_id.startswith("AntMaze_"):
+            kw["ant_version"] = int(env_id[-1])
         register(id=env_id, vector_entry_point=ep, kwargs=kw)
     return True

@@ -60,6 +60,14 @@ class ReachResetC(ctypes.Structure):
     _fields_ = [("meeting", ctypes.c_float * 3), ("initial_goal", ctypes.c_float * 15)]
 
 
+class AntParamsC(ctypes.Structure):
+    """b200sim_ant_params_t"""
+    _fields_ = [("version", ctypes.c_int)] + [(n, ctypes.c_float) for n in ("forward_reward_weight", "ctrl_cost_weight", "contact_cost_weight",
+                                                                           "healthy_reward")] + \
+               [("terminate_when_unhealthy", ctypes.c_int), ("use_contact_forces", ctypes.c_int), ("healthy_z_range", ctypes.c_float * 2),
+                ("contact_force_range", ctypes.c_float * 2)]
+
+
 class KeepC(ctypes.Structure):
     """b200sim_keep_t"""
     _fields_ = [("n", ctypes.c_int), ("start", ctypes.c_int * 4), ("len", ctypes.c_int * 4)]
@@ -68,7 +76,7 @@ class KeepC(ctypes.Structure):
 def build_library(force: bool = False, verbose: bool = False) -> str:
     """nvcc-compile csrc/b200sim.cu and csrc/b200sim_wide.cu for sm_90a into the in-tree libb200sim.so (cross-compiles
     without a GPU; the two translation units are compiled in parallel)."""
-    names = ("b200sim", "b200sim_wide", "b200sim_kitchen", "b200sim_kitchen_groups", "b200sim_kitchen_hull")
+    names = ("b200sim", "b200sim_wide", "b200sim_kitchen", "b200sim_kitchen_groups", "b200sim_kitchen_hull", "b200sim_ant")
     srcs = [os.path.join(_HERE, "csrc", n + ".cu") for n in names]
     deps = srcs + [os.path.join(_HERE, "csrc", f) for f in ("sim_core.cuh", "fetch_task.cuh", "step_kernel.cuh", "dmodel.h", "reset_sample.cuh")] + \
            [os.path.join(_HERE, "..", "include", f) for f in ("b200sim.h", "b200sim_model.h")]
@@ -126,6 +134,7 @@ def lib():
     L.b200sim_reset_uniform.argtypes = [vp, vp, vp, ctypes.POINTER(UniformResetC), ctypes.c_ulonglong, ci, vp] + [vp] * 6
     L.b200sim_set_obs_noise.argtypes = [vp, vp, ctypes.c_ulonglong, ci, vp]
     L.b200sim_set_goal_update.argtypes = [vp, vp, ci, ctypes.c_float, ctypes.c_float, ctypes.c_ulonglong, ci, vp]
+    L.b200sim_set_ant_info.argtypes = [vp, ctypes.POINTER(AntParamsC), vp, vp]
     L.b200sim_launch_count.argtypes = [vp]
     L.b200sim_launch_count.restype = ctypes.c_long
     L.b200sim_launch_config.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)]
@@ -134,6 +143,6 @@ def lib():
 
 
 EXPORTED_SYMBOLS = ["b200sim_create", "b200sim_destroy", "b200sim_last_error", "b200sim_num_envs", "b200sim_layout",
-                    "b200sim_state", "b200sim_step", "b200sim_refresh", "b200sim_raw_step", "b200sim_raw_step_masked", "b200sim_compute_reward", "b200sim_reset", "b200sim_reset_uniform", "b200sim_reset_maze", "b200sim_check_state", "b200sim_reset_reach", "b200sim_reset_hand_pose", "b200sim_reset_hand_goal", "b200sim_set_obs_noise", "b200sim_set_goal_update",
+                    "b200sim_state", "b200sim_step", "b200sim_refresh", "b200sim_raw_step", "b200sim_raw_step_masked", "b200sim_compute_reward", "b200sim_reset", "b200sim_reset_uniform", "b200sim_reset_maze", "b200sim_check_state", "b200sim_reset_reach", "b200sim_reset_hand_pose", "b200sim_reset_hand_goal", "b200sim_set_obs_noise", "b200sim_set_goal_update", "b200sim_set_ant_info",
                     "b200sim_launch_count", "b200sim_launch_config", "b200sim_set_time_limit", "b200sim_elapsed", "b200sim_overflow_counter",
                     "b200sim_packed_width", "b200sim_set_packed"]

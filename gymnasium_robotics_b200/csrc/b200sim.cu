@@ -151,6 +151,8 @@ extern const KernelUnit kernel_unit_wide;
 // b200sim_kitchen_hull.cu (the groups build + support-map narrow phase for MESH geoms, models compiled with mesh_hull)
 extern const KernelUnit kernel_unit_kitchen, kernel_unit_kitchen_groups, kernel_unit_kitchen_hull;
 #define B200_KITCHEN_NVP 31   // the kitchen translation units instantiate NVP = 31 (identity-padded; distinct kernel symbols)
+// the ant build (b200sim_ant.cu): maze handles with touch_mode 2..4, the Ant's keywords and per-step info (b200sim_set_ant_info)
+extern const KernelUnit kernel_unit_ant;
 
 struct b200sim {
   int N = 0, device = 0;
@@ -167,6 +169,8 @@ struct b200sim {
   int packed = 0, packed_w = 0;                  // b200sim_set_packed
   ObsNoiseArgs noise = {nullptr, nullptr, 0, 0};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
   GoalUpdateArgs goal_update = {nullptr, 0, 0.f, 0.f, 0, 0, nullptr};   // b200sim_set_goal_update (maze tasks)
+  // b200sim_set_ant_info (ant build): Ant-v5's defaults, no info rows until set
+  AntInfoArgs ant = {-1.f, 1.f, 1.f, 0.5f, 5e-4f, 1.f, 0.2f, 1.f, 0, 0, 0, nullptr, nullptr};
   size_t smem_bytes = 0;
   int blocks = 0;
   long launches = 0;
@@ -230,7 +234,7 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   const char* groups = getenv("B200SIM_KITCHEN_GROUPS");   // default: two-level broad phase
   h->unit = hull ? &kernel_unit_kitchen_hull
                  : kitchen ? (groups && groups[0] && atoi(groups) == 0 ? &kernel_unit_kitchen : &kernel_unit_kitchen_groups)
-                           : (v.nv > 32 ? &kernel_unit_wide : &kernel_unit_plain);
+                           : (v.nv > 32 ? &kernel_unit_wide : (task->kind == TASK_ANTMAZE && task->touch_mode >= 2 ? &kernel_unit_ant : &kernel_unit_plain));
   const int penv = TASK_IS_ADROIT(task->kind) ? task->penv_body : -1;
   if (h->unit->build(v, eq_data, r, penv, h->model_host, err) != 0) { delete h; return fail(nullptr, "b200sim_create: " + err, -4); }
   const DMHead* dh = (const DMHead*)h->model_host.data();
@@ -281,8 +285,9 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
                               t.touch_mode < 0 || t.touch_mode > 3 || (t.touch_mode && dh->nsensor == 0) ||
                               t.nobs != t.obj_qadr + dh->nv + 7 + (t.touch_mode ? dh->nsensor : 0))) { delete h; return fail(nullptr, "b200sim_create: inconsistent Hand task", -6); }
   if (t.kind == TASK_FETCH && dh->nmocap != 1) { delete h; return fail(nullptr, "b200sim_create: Fetch task needs exactly one mocap body", -6); }
-  if (t.kind == TASK_ANTMAZE && (t.nact != dh->nu || t.ngoal != 2 || t.touch_mode < 0 || t.touch_mode > 1 ||
-                                 t.nobs != dh->nq - t.obs_qpos_start + dh->nv + (t.touch_mode == 1 ? 6 * (dh->nmjb - 1) : 0))) { delete h; return fail(nullptr, "b200sim_create: inconsistent AntMaze task", -6); }
+  if (t.kind == TASK_ANTMAZE && (t.nact != dh->nu || t.ngoal != 2 || t.touch_mode < 0 || t.touch_mode > 4 ||
+                                 t.nobs != dh->nq - t.obs_qpos_start + dh->nv + (t.touch_mode == 1 || t.touch_mode == 3 ? 6 * (dh->nmjb - 1) :
+                                                                                 (t.touch_mode == 4 ? 6 * dh->nmjb : 0)))) { delete h; return fail(nullptr, "b200sim_create: inconsistent AntMaze task", -6); }
   if (t.kind == TASK_HAND_REACH) {
     bool ok = t.nact == dh->nu && t.ngoal == 15 && t.nobs == dh->nq + dh->nv + 15;
     for (int k = 0; k < 5; k++) ok = ok && t.tip_site[k] >= 0 && t.tip_site[k] < dh->nsite;
@@ -293,6 +298,7 @@ int b200sim_create(const void* model_blob, size_t nbytes, const double* eq_data,
   t.st_mocap = o; o += 7 * dh->nmocap; t.st_pose = o; o += (t.kind == TASK_FETCH ? 7 : 0); t.st_goal = o; o += t.ngoal;
   t.st_penv = o; o += (t.penv_body > 0 ? 7 : 0);
   t.st_stride = (o + 3) & ~3;
+  if (h->unit == &kernel_unit_ant && t.st_stride - o < 2) { delete h; return fail(nullptr, "b200sim_create: no spare record words for the ant build's torso position", -6); }
   DevGuard guard(device);
   if (!guard.ok) { delete h; return fail(nullptr, "b200sim_create: cudaSetDevice failed", -7); }
   int nsm = 132;
@@ -408,7 +414,7 @@ static int launch(b200sim* h, int mode, int nraw, const float* actions, const un
   io.terminated = terminated; io.truncated = truncated; io.info = info;
   io.elapsed = h->elapsed; io.max_steps = h->max_steps; io.term_on_success = h->term_on_success; io.overflow_count = h->overflow_count;
   ON_DEVICE(h);
-  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io, h->noise))
+  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io, h->noise, h->ant))
     return fail(h, "no kernel variant for this (envs per block, nv) pair: nothing was launched", -8);
   h->launches++;
   CUDA_OK(cudaGetLastError());
@@ -435,6 +441,17 @@ int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, floa
   if (goal_xy && n_goal < 2) return fail(h, "b200sim_set_goal_update: fewer than two goal cells", -1);
   if (env_offset < 0) return fail(h, "b200sim_set_goal_update: negative env_offset", -1);
   h->goal_update = goal_xy ? GoalUpdateArgs{goal_xy, n_goal, scaling, noise, seed, env_offset, episode} : GoalUpdateArgs{nullptr, 0, 0.f, 0.f, 0, 0, nullptr};
+  return 0;
+}
+int b200sim_set_ant_info(b200sim_t* h, const b200sim_ant_params_t* p, float* rows, const float* origin) {
+  if (h->unit != &kernel_unit_ant) return fail(h, "b200sim_set_ant_info: not an ant-build handle (maze task with touch_mode 2..4)", -6);
+  if (!p || (p->version != 4 && p->version != 5)) return fail(h, "b200sim_set_ant_info: params NULL or version not 4 / 5", -1);
+  if (!(p->contact_force_range[0] <= p->contact_force_range[1])) return fail(h, "b200sim_set_ant_info: contact_force_range is not (min, max)", -1);
+  if (rows && p->version == 5 && !origin) return fail(h, "b200sim_set_ant_info: Ant-v5 info needs origin", -1);
+  const bool v4 = p->version == 4;
+  h->ant = {p->contact_force_range[0], p->contact_force_range[1], v4 ? 1.f : p->forward_reward_weight, p->ctrl_cost_weight, p->contact_cost_weight,
+            p->healthy_reward, p->healthy_z_range[0], p->healthy_z_range[1], v4 ? 1 : 0, v4 && p->terminate_when_unhealthy ? 1 : 0,
+            v4 && p->use_contact_forces ? 1 : 0, rows, origin};
   return 0;
 }
 int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long seed, int env_offset, const int* episode) {

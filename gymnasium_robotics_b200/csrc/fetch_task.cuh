@@ -135,6 +135,11 @@ HD void fetch_observe(const Ctx& c, const FetchTask& t, const float* goal, float
   }
 }
 
+#ifdef B200_ANT
+// The ant build's contact forces (b200sim_set_ant_info): the clip range contact_force_range in, the warp's sum of the squares of the
+// clipped forces of every body out (the contact cost's; the world row is zero)
+struct AntForces { float lo, hi, sq; };
+#endif
 // AntMaze: obs = ant qpos[2:] | qvel [| clipped contact forces], achieved = qpos[:2]; reward exp(-d) (dense) or d <= r (sparse)
 // (reference: envs/maze/ant_maze_v5.py:295-320, envs/maze/maze_v4.py:381-398).
 // touch_mode == 1 (AntMaze-v5 on Gymnasium's Ant-v5 [ext], ant_maze_v5.py:99: observation (105,) = 27 + 13 x 6): appended are the
@@ -144,13 +149,33 @@ HD void fetch_observe(const Ctx& c, const FetchTask& t, const float* goal, float
 // spatial force about `ref` is sum_k F_k w_k over its contacts' base rows (what pass_F feeds into J^T f); body B of the pair
 // receives +, body A -.  A refresh (no sub-step) reports zeros, as the reference's reset observation does (mj_resetData).
 HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, float* obs, float* achieved, float* desired,
-                        float* reward, float* success, bool stepped) {
+                        float* reward, float* success, bool stepped
+#ifdef B200_ANT
+                        , AntForces* ant = nullptr
+#endif
+                        ) {
   const DMHead* h = c.h;
   const int q0 = t.obs_qpos_start;
   LANES(i, h->nq - q0) obs[i] = SF(qpos)[q0 + i];
   LANES(i, h->nv) obs[h->nq - q0 + i] = SF(qvel)[i];
+#ifdef B200_ANT
+  // touch_mode 3: cfrc_ext[1:] appended (Ant-v5), 4: all of cfrc_ext, world row first (Ant-v4 use_contact_forces, (111,)), 2: none; the
+  // forces are clipped to contact_force_range and computed in every case, for the contact cost (the sum of their squares)
+  const float cf_lo = ant ? ant->lo : -1.f, cf_hi = ant ? ant->hi : 1.f;
+  float* cf = t.touch_mode >= 3 ? obs + (h->nq - q0 + h->nv) : nullptr;
+  if (t.touch_mode == 4) { LANES(k, 6) cf[k] = 0.f; cf += 6; }
+  float cf_sq = 0.f;
+#define B200_CF_PUT(dst, v) do { const float v_ = (v); if (cf) dst = v_; cf_sq += v_ * v_; } while (0)
+#define B200_CF_LO cf_lo
+#define B200_CF_HI cf_hi
+  {
+#else
+#define B200_CF_PUT(dst, v) dst = v
+#define B200_CF_LO -1.f
+#define B200_CF_HI 1.f
   if (t.touch_mode == 1) {
     float* cf = obs + (h->nq - q0 + h->nv);
+#endif
     const int* cnt = SI(counters);
     const int ngrp = stepped ? cnt[CNT_NGRP] : 0;
     LANES(i, stepped ? cnt[CNT_NCON] : 0) {   // base-row forces of every contact (parked in the JV slots, as pass_F does)
@@ -177,7 +202,7 @@ HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, flo
     SYNC();
     LANES(b1, h->nmjb - 1) {
       if (!stepped) {   // a refresh computes no kinematics: xpos / xquat below would be whatever the shared memory last held
-        for (int k = 0; k < 6; k++) cf[6 * b1 + k] = 0.f;
+        for (int k = 0; k < 6; k++) B200_CF_PUT(cf[6 * b1 + k], 0.f);
         continue;
       }
       const int b = b1 + 1;      // MJCF body: the row layout of data.cfrc_ext (fused bodies keep their own rows)
@@ -205,11 +230,17 @@ HD void antmaze_observe(const Ctx& c, const FetchTask& t, const float* goal, flo
       for (int a = 0; a < 3; a++) off[a] = com[a] / mass - h->ref[a];
       cross3(tq, off, acc + 3);   // torque about the com = torque about ref - (com - ref) x force
       for (int a = 0; a < 3; a++) {
-        cf[6 * b1 + a] = fminf(fmaxf(acc[a] - tq[a], -1.f), 1.f);
-        cf[6 * b1 + 3 + a] = fminf(fmaxf(acc[3 + a], -1.f), 1.f);
+        B200_CF_PUT(cf[6 * b1 + a], fminf(fmaxf(acc[a] - tq[a], B200_CF_LO), B200_CF_HI));
+        B200_CF_PUT(cf[6 * b1 + 3 + a], fminf(fmaxf(acc[3 + a], B200_CF_LO), B200_CF_HI));
       }
     }
   }
+#ifdef B200_ANT
+  if (ant) ant->sq = wsum(cf_sq);
+#endif
+#undef B200_CF_PUT
+#undef B200_CF_LO
+#undef B200_CF_HI
   if (c.lane == 0) {
     float dx = SF(qpos)[0] - goal[0], dy = SF(qpos)[1] - goal[1];
     // the same rounding sequence as reward_kernel's loop over the goal entries (b200sim.cu): round(dx^2), then one fused multiply-add --
@@ -593,12 +624,16 @@ HD void kitchen_observe(const Ctx& c, const FetchTask& t, float* obs, float* ach
 // one env, one warp.  `st` is this env's state record; outputs are this env's rows.  `active` is warp-uniform: idle
 // warps run the same control flow (for the block-wide alignment barriers) but touch no memory.
 // REBUILD: rebuild the context before each stage call (stage_ctx).  Kitchen builds: `noise`, the env's observation noise (NULL =
-// none); the parameter exists in those builds only, so that the other builds' kernels keep their source and parameters.
+// none); the ant build: `ant`, the contact-force clip range in, the contact forces' sum of squares out; these parameters exist in
+// those builds only, so that the other builds' kernels keep their source and parameters.
 template <int NVP, bool REBUILD = false>
 HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, int nraw, float* st, const float* action, float* obs,
                        float* achieved, float* desired, float* reward, float* success, int* iters_out
 #ifdef B200_KITCHEN
                        , const ObsNoiseKey* noise = nullptr
+#endif
+#ifdef B200_ANT
+                       , AntForces* ant = nullptr
 #endif
                        ) {
   const DMHead* h = c.h;
@@ -685,8 +720,64 @@ HD void fetch_env_step(const Ctx& c, const FetchTask& t, bool active, int mode, 
     hand_observe(c, t, st + t.st_goal, obs, achieved, desired, reward, success);
     if (t.touch_mode) touch_observe(c, t, obs + t.obj_qadr + h->nv + 7);
   } else {
+#ifdef B200_ANT
+    antmaze_observe(c, t, st + t.st_goal, obs, achieved, desired, reward, success, nsub > 0, ant);
+#else
     antmaze_observe(c, t, st + t.st_goal, obs, achieved, desired, reward, success, nsub > 0);
+#endif
   }
   store_state(c, t, st);
   if (iters_out && c.lane == 0) *iters_out = SI(counters)[CNT_ITERS] | (SI(counters)[CNT_OVERFLOW] << 16);
 }
+
+// The Ant's keywords and per-step info of a handle (b200sim_set_ant_info): contact_force_range, the cost and reward weights, the healthy
+// z range, the Ant version's info rules, the [N, 9] info rows (NULL = none) and the [N, 2] reset positions of Ant-v5's
+// distance_from_origin.  A kernel parameter of the ant build only (b200sim_ant.cu, csrc/step_kernel.cuh), as ObsNoiseArgs is of the kitchen builds.
+struct AntInfoArgs {
+  float cf_lo, cf_hi, forward_w, ctrl_w, contact_w, healthy_reward, z_lo, z_hi;
+  int v4, survive_always, contact_in_ctrl;   // Ant-v4 rules; terminate_when_unhealthy and use_contact_forces under them
+  float* rows; const float* origin;
+};
+#ifdef B200_ANT
+// Lane 0 of an ant-build env after its launch.  The torso's xy of the last forward pass (the last RK4 stage of a step; qpos[0:2] after a
+// refresh, which runs mj_forward on the new state) is kept in the two record words after the goal; a step's velocity is the change of
+// it over dt = timestep x frame_skip.  A step writes the info row of Ant.step [ext] (ant_v3.py:76-145 with the v4 / v5 changes): v5
+// x, y = qpos[0:2], distance from the reset position, reward_forward = forward_reward_weight * vx, reward_ctrl = -ctrl_cost (the
+// action as passed, before the ctrlrange clamp), reward_contact = -contact_cost, reward_survive = healthy_reward * is_healthy; v4 x, y
+// = the torso's xpos and its distance from the world origin, reward_forward = vx, reward_ctrl = -contact_cost under
+// use_contact_forces (Ant-v4's info bug, fixed in v5), reward_survive = healthy_reward * (is_healthy or terminate_when_unhealthy).  A
+// refresh writes the reset info (v5: x, y and distance 0; v4: none) with the other columns 0.
+HD void ant_info(const Ctx& c, const FetchTask& t, const AntInfoArgs& a, int mode, bool stepped, float* st, const float* action,
+                 float contact_sq, size_t e) {
+  const DMHead* h = c.h;
+  const float* qp = SF(qpos);
+  float* stale = st + t.st_goal + t.ngoal;
+  const int tb = 3 * GI(mjb_rt)[1];   // MJCF body 1, the torso (main_body)
+  const float x = stepped ? SF(xpos)[tb] : qp[0], y = stepped ? SF(xpos)[tb + 1] : qp[1];
+  if (a.rows && mode != MODE_RAW) {
+    float r[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (mode == MODE_STEP) {
+      const float vx = (x - stale[0]) / t.dt, vy = (y - stale[1]) / t.dt;
+      float ctrl = 0.f;
+      for (int i = 0; i < t.nact; i++) ctrl += action[i] * action[i];
+      ctrl *= a.ctrl_w;
+      const float contact = a.contact_w * contact_sq;
+      bool healthy = qp[2] >= a.z_lo && qp[2] <= a.z_hi;
+      for (int i = 0; i < h->nq; i++) healthy = healthy && isfinite(qp[i]);
+      for (int i = 0; i < h->nv; i++) healthy = healthy && isfinite(SF(qvel)[i]);
+      r[3] = vx; r[4] = vy; r[7] = -contact;
+      r[8] = (healthy || (a.v4 && a.survive_always)) ? a.healthy_reward : 0.f;
+      if (a.v4) {
+        r[0] = x; r[1] = y; r[2] = sqrtf(x * x + y * y); r[5] = vx; r[6] = a.contact_in_ctrl ? -contact : -ctrl;
+      } else {
+        const float dx = qp[0] - a.origin[2 * e], dy = qp[1] - a.origin[2 * e + 1];
+        r[0] = qp[0]; r[1] = qp[1]; r[2] = sqrtf(dx * dx + dy * dy); r[5] = a.forward_w * vx; r[6] = -ctrl;
+      }
+    } else if (!a.v4) {
+      r[0] = qp[0]; r[1] = qp[1];
+    }
+    for (int k = 0; k < 9; k++) a.rows[9 * e + k] = r[k];
+  }
+  stale[0] = x; stale[1] = y;
+}
+#endif

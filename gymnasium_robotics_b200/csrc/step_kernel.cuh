@@ -1,7 +1,7 @@
 // The step kernel: one warp integrates one env for a whole env-step (all sub-steps on chip); WPB warps share one copy of
 // the model constants that a single thread stages into shared memory with a TMA bulk copy (cp.async.bulk + mbarrier).
 // Included by each kernel build (translation unit): b200sim.cu (32-bit dof masks, NVP <= 30), b200sim_wide.cu (B200_WIDE: 64-bit
-// dof masks, NVP = 36) and the three b200sim_kitchen*.cu; each one names its instantiations once, in B200_KERNEL_UNIT.
+// dof masks, NVP = 36), the three b200sim_kitchen*.cu and b200sim_ant.cu (B200_ANT); each one names its instantiations once, in B200_KERNEL_UNIT.
 #pragma once
 #include <cuda_runtime.h>
 #include "fetch_task.cuh"
@@ -38,6 +38,9 @@ struct ObsNoiseArgs {
 #ifdef B200_KITCHEN
 #define B200_KITCHEN_PARAM , ObsNoiseArgs noise_args
 #define B200_KITCHEN_ARG , noise_args
+#elif defined(B200_ANT)
+#define B200_KITCHEN_PARAM , AntInfoArgs ant_args
+#define B200_KITCHEN_ARG , ant_args
 #else
 #define B200_KITCHEN_PARAM
 #define B200_KITCHEN_ARG
@@ -96,6 +99,13 @@ __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restr
                                  noisy ? (uint32_t)(io.elapsed[e] + (mode == MODE_STEP ? 1 : 0)) : 0u};
   fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
                       io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters, noisy ? &noise_key : nullptr);
+#elif defined(B200_ANT)
+  AntForces antf = {ant_args.cf_lo, ant_args.cf_hi, 0.f};
+  fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
+                      io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters, &antf);
+  if (active && lane == 0)
+    ant_info(c, task, ant_args, mode, mode == MODE_STEP ? task.n_substeps > 0 : (mode == MODE_RAW && nraw > 0), io.state + e * task.st_stride, act,
+             antf.sq, e);
 #else
   // (WPB >= 28: at most 72 registers per thread, the driver rebuilds its context before each stage call -- stage_ctx)
   fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
@@ -133,8 +143,8 @@ struct KernelUnit {
   bool (*has)(int wpb, int nvp);                                // an instantiation <wpb, nvp> exists
   cudaError_t (*setattr)(int wpb, int nvp, int smem_bytes);     // cudaErrorInvalidValue when it does not
   bool (*launch)(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev, const FetchTask& task,
-                 int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args);  // false (nothing launched) when it does not;
-};                                                                                                  // noise_args reach the kitchen units' kernels only
+                 int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args, const AntInfoArgs& ant_args);
+};   // launch: false (nothing launched) when it does not; noise_args reach the kitchen units' kernels only, ant_args the ant unit's
 
 #define B200_UNIT_HAS(W, V) || (wpb == W && nvp == V)
 #define B200_UNIT_SETATTR(W, V) \
@@ -157,7 +167,8 @@ struct KernelUnit {
     return cudaErrorInvalidValue;                                                                                                    \
   }                                                                                                                                  \
   static bool unit_launch(int wpb, int nvp, int blocks, size_t smem_bytes, cudaStream_t stream, const uint32_t* model_dev,           \
-                          const FetchTask& task, int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args) {      \
+                          const FetchTask& task, int mode, int nraw, int N, const StepIO& io, const ObsNoiseArgs& noise_args,        \
+                          const AntInfoArgs& ant_args) {                                                                             \
     VARIANTS(B200_UNIT_LAUNCH)                                                                                                       \
     return false;                                                                                                                    \
   }                                                                                                                                  \

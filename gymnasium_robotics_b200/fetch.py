@@ -203,6 +203,15 @@ class CudaBackend:
                                                    float(noise), int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset),
                                                    episode.data_ptr() if on else None))
 
+    def set_ant_info(self, params, rows, origin):
+        """b200sim_set_ant_info (ant-build handles): the Ant's keywords, and the [N, 9] info rows later launches write (None: no rows)
+        with the [N, 2] Ant-v5 reset positions.  The handle keeps both pointers: the tensors must outlive its launches."""
+        for t, w in ((rows, 9), (origin, 2)):
+            if t is not None:
+                assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == (self.num_envs, w)
+        self._check(self.L.b200sim_set_ant_info(self.h, ctypes.byref(params), rows.data_ptr() if rows is not None else None,
+                                                origin.data_ptr() if origin is not None else None))
+
     def reset_maze(self, mask, rest_record, params, goal_xy, reset_xy, seed, env_offset, episode, out):
         """b200sim_reset_maze: goal cell + noise, reset cell away from the goal + noise, then mj_forward + _get_obs."""
         assert rest_record.is_cuda and rest_record.dtype == torch.float32 and rest_record.numel() == self.layout["stride"]

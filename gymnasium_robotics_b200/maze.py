@@ -124,18 +124,100 @@ def check_maze_map(maze_map, scaling):
     return rows
 
 
-def make_maze_task(model, reward_type, agent="ant", contact_forces=False):
-    """contact_forces: append Ant-v5's clipped `cfrc_ext[1:]` (6 values per body) to the observation -- (105,) instead of (27,)"""
+def make_maze_task(model, reward_type, agent="ant", contact_forces=False, frame_skip=None, touch_mode=None):
+    """contact_forces: append Ant-v5's clipped `cfrc_ext[1:]` (6 values per body) to the observation -- (105,) instead of (27,).
+    touch_mode (the Ant's keywords, `AntKeywords.touch_mode`) overrides it: 2..4 select the ant kernel build, 4 appends all of
+    `cfrc_ext`, world row included -- Ant-v4's (111,)."""
     cfg = AGENTS[agent]
+    frame_skip = cfg["frame_skip"] if frame_skip is None else frame_skip
+    mode = int(bool(contact_forces)) if touch_mode is None else touch_mode
     t = _lib.FetchTaskC()
     t.kind, t.nact, t.ngoal = 1, int(model.nu), 2
-    t.n_substeps, t.reward_dense = cfg["frame_skip"], int(reward_type == "dense")
+    t.n_substeps, t.reward_dense = frame_skip, int(reward_type == "dense")
     t.obs_qpos_start, t.vel_clip = cfg["obs_qpos_start"], cfg["vel_clip"]
-    t.touch_mode = int(bool(contact_forces))
-    t.nobs = int(model.nq - cfg["obs_qpos_start"] + model.nv) + (6 * (len(model.mjbody_rt) - 1) if contact_forces else 0)
+    t.touch_mode = mode
+    nmjb = len(model.mjbody_rt)
+    t.nobs = int(model.nq - cfg["obs_qpos_start"] + model.nv) + {1: 6 * (nmjb - 1), 3: 6 * (nmjb - 1), 4: 6 * nmjb}.get(mode, 0)
     t.success_radius = SUCCESS_RADIUS
-    t.dt = float(model.opt[0] * cfg["frame_skip"])
+    t.dt = float(model.opt[0] * frame_skip)
     return t
+
+
+# The info keys of the Ant (Ant.step [ext]), in the column order of the [N, 9] info rows the ant kernel build writes
+# (b200sim_set_ant_info)
+ANT_INFO_COLUMNS = ("x_position", "y_position", "distance_from_origin", "x_velocity", "y_velocity", "reward_forward", "reward_ctrl",
+                    "reward_contact", "reward_survive")
+# Gymnasium's Ant-v5 / Ant-v4 keywords [ext] that the maze forwards to its AntEnv (ant_maze_v5.py:249-255, ant_maze_v4.py:62-67) and
+# their defaults.  AntMaze passes reset_noise_scale and exclude_current_positions_from_observation itself, so the reference refuses
+# them with a TypeError; so are the keywords that the other version's AntEnv does not take.
+ANT_KEYWORDS = {
+    5: dict(frame_skip=5, forward_reward_weight=1.0, ctrl_cost_weight=0.5, contact_cost_weight=5e-4, healthy_reward=1.0, main_body=1,
+            terminate_when_unhealthy=True, healthy_z_range=(0.2, 1.0), contact_force_range=(-1.0, 1.0), include_cfrc_ext_in_observation=True),
+    4: dict(ctrl_cost_weight=0.5, use_contact_forces=False, contact_cost_weight=5e-4, healthy_reward=1.0, terminate_when_unhealthy=True,
+            healthy_z_range=(0.2, 1.0), contact_force_range=(-1.0, 1.0)),
+}
+
+
+class AntKeywords:
+    """The Ant keywords of one AntMaze env: parsed, refused as the reference refuses them, and turned into the kernel's settings."""
+
+    def __init__(self, version, kwargs, include_cfrc):
+        if version not in ANT_KEYWORDS:
+            raise ValueError(f"ant_version must be 4 or 5, got {version!r}")
+        for k in ("reset_noise_scale", "exclude_current_positions_from_observation"):
+            if k in kwargs:
+                raise TypeError(f"AntEnv got multiple values for keyword argument {k!r} (AntMaze passes it itself)")
+        if "xml_file" in kwargs:
+            if version == 4:
+                raise TypeError("AntEnv got multiple values for keyword argument 'xml_file' (AntMaze-v4 passes it itself)")
+            raise NotImplementedError("xml_file: the CUDA build steps the committed ant model only")
+        other = ANT_KEYWORDS[9 - version]
+        for k in list(kwargs):
+            if k in other and k not in ANT_KEYWORDS[version]:
+                raise TypeError(f"Ant-v{version} got an unexpected keyword argument {k!r}")
+        if version == 4 and include_cfrc is not None:
+            raise TypeError("Ant-v4 got an unexpected keyword argument 'include_cfrc_ext_in_observation'")
+        kw = dict(ANT_KEYWORDS[version])
+        self.frame_skip_given = "frame_skip" in kwargs
+        kw.update({k: kwargs.pop(k) for k in list(kwargs) if k in kw})
+        kw["include_cfrc_ext_in_observation"] = bool(include_cfrc) if version == 5 else False
+        if version == 5 and kw["main_body"] not in (1, "torso"):
+            raise NotImplementedError(f"main_body={kw['main_body']!r}: the CUDA build measures the torso (main_body 1) only")
+        frame_skip = kw.get("frame_skip", 5)
+        if isinstance(frame_skip, bool) or not isinstance(frame_skip, (int, np.integer)) or frame_skip < 1:
+            raise ValueError(f"frame_skip must be a positive integer, got {frame_skip!r}")
+        lo, hi = (float(v) for v in kw["contact_force_range"])
+        if not lo <= hi:
+            raise ValueError(f"contact_force_range must be (min, max), got {kw['contact_force_range']!r}")
+        self.version, self.kw, self.frame_skip, self.cf_range = version, kw, int(frame_skip), (lo, hi)
+        self.contact_obs = kw["include_cfrc_ext_in_observation"] or bool(kw.get("use_contact_forces", False))
+
+    def needs_ant_build(self, ant_info):
+        """The plain kernel build observes cfrc_ext[1:] clipped to (-1, 1) or nothing; anything else runs the ant build."""
+        return ant_info or self.version == 4 and self.contact_obs or self.contact_obs and self.cf_range != (-1.0, 1.0)
+
+    def touch_mode(self, ant_info):
+        if not self.needs_ant_build(ant_info):
+            return int(self.contact_obs)
+        return 4 if self.version == 4 and self.contact_obs else (3 if self.contact_obs else 2)
+
+    def params(self):
+        kw, p = self.kw, _lib.AntParamsC()
+        p.version = self.version
+        p.forward_reward_weight = float(kw.get("forward_reward_weight", 1.0))
+        p.ctrl_cost_weight, p.contact_cost_weight, p.healthy_reward = (float(kw[k]) for k in ("ctrl_cost_weight", "contact_cost_weight", "healthy_reward"))
+        p.terminate_when_unhealthy, p.use_contact_forces = int(bool(kw["terminate_when_unhealthy"])), int(bool(kw.get("use_contact_forces", False)))
+        p.healthy_z_range[0], p.healthy_z_range[1] = (float(v) for v in kw["healthy_z_range"])
+        p.contact_force_range[0], p.contact_force_range[1] = self.cf_range
+        return p
+
+    def info_keys(self):
+        """(step keys, reset keys) as (name, column) pairs: Ant-v5's, or Ant-v4's (no reward_contact, forward_reward = reward_forward)."""
+        col = {k: i for i, k in enumerate(ANT_INFO_COLUMNS)}
+        if self.version == 5:
+            return tuple(col.items()), tuple((k, col[k]) for k in ANT_INFO_COLUMNS[:3])
+        step = tuple((k, c) for k, c in col.items() if k != "reward_contact") + (("forward_reward", col["reward_forward"]),)
+        return step, ()
 
 
 def make_antmaze_task(model, reward_type):
@@ -159,16 +241,22 @@ class MazeVectorEnv(VectorEnv):
     def __init__(self, maze="Large", num_envs: int = 1, reward_type: str = "sparse", continuing_task: bool = True,
                  reset_target: bool = False, max_episode_steps: Optional[int] = None, device="cuda:0", rng_mode: str = "auto",
                  autoreset_mode: str = "next_step", backend_factory=None, agent: Optional[str] = None, model=None,
-                 include_cfrc_ext_in_observation: bool = False, maze_map=None, **kwargs):
+                 include_cfrc_ext_in_observation: Optional[bool] = None, maze_map=None, ant_version: Optional[int] = None,
+                 ant_info: bool = False, **kwargs):
         self.agent = agent or self.AGENT
         cfg = AGENTS[self.agent]
+        # the Ant's keywords (Gymnasium's Ant-v5 for the -v5 ids and by default, Ant-v4 for the -v4 ids); they leave `kwargs`
+        self.ant = AntKeywords(5 if ant_version is None else ant_version, kwargs, include_cfrc_ext_in_observation) if self.agent == "ant" else None
+        if self.ant is None and (ant_info or ant_version is not None):
+            raise ValueError("ant_version / ant_info are keywords of the ant agent")
+        self.ant_info = bool(ant_info)
         if isinstance(maze, str) and maze not in MAPS:
             raise KeyError(f"unknown maze {maze!r}")
         if reward_type not in ("sparse", "dense"):
             raise ValueError("reward_type must be 'sparse' or 'dense'")
         self.maze_name, self.reward_type = maze, reward_type
         self.continuing_task, self.reset_target = continuing_task, reset_target
-        self.scaling, self.frame_skip = cfg["scaling"], cfg["frame_skip"]
+        self.scaling, self.frame_skip = cfg["scaling"], (self.ant.frame_skip if self.ant else cfg["frame_skip"])
         named = isinstance(maze, str)
         if maze_map is not None:
             if not named:
@@ -186,7 +274,7 @@ class MazeVectorEnv(VectorEnv):
         # Ant-v5 keyword [ext]: AntMaze_*-v5 observes the clipped per-body contact forces (ant_maze_v5.py:99: (105,) = 27 + 13 x 6);
         # AntMaze_*-v4 (Ant-v4, use_contact_forces False) and the point agent do not.  The registry sets it per id.
         self.include_cfrc = bool(include_cfrc_ext_in_observation) and self.agent == "ant"
-        t = make_maze_task(m, reward_type, self.agent, self.include_cfrc)
+        t = make_maze_task(m, reward_type, self.agent, self.include_cfrc, self.frame_skip, self.ant.touch_mode(self.ant_info) if self.ant else None)
         box = lambda n: Box(-np.inf, np.inf, shape=(n,), dtype=np.float64)
         # "device": goal / reset cells and their noise are drawn inside the library (b200sim_reset_maze, csrc/reset_sample.cuh).
         # TimeLimit and compute_terminated (maze_v4.py:390-398: success ends the episode unless continuing_task) run inside the
@@ -198,7 +286,18 @@ class MazeVectorEnv(VectorEnv):
                          max_episode_steps=(cfg["steps"][maze] if named else None) if max_episode_steps is None else max_episode_steps,
                          autoreset_mode=autoreset_mode, rng_mode=rng_mode, n_substeps=self.frame_skip, kwargs=kwargs,
                          terminate_on_success=not continuing_task)
-        self.metadata["render_fps"] = cfg["fps"]
+        # the Ant's frame_skip: the inner AntEnv's render rate (MujocoEnv: round(1 / dt))
+        self.metadata["render_fps"] = int(round(1.0 / self.dt)) if self.ant is not None and self.ant.frame_skip_given else cfg["fps"]
+        # the ant kernel build (b200sim_set_ant_info): the Ant's keywords; with ant_info a fresh [N, 9] info row buffer per call
+        # (_new_ant_rows) and the reset positions Ant-v5 measures distance_from_origin from
+        self._ant_rows = self._ant_origin = None
+        if self.ant is not None and t.touch_mode >= 2:
+            if not hasattr(self.backend, "set_ant_info"):
+                raise NotImplementedError(f"{type(self.backend).__name__} cannot run the Ant's keywords (no set_ant_info)")
+            self._ant_params = self.ant.params()
+            self._ant_origin = torch.zeros((self.num_envs, 2), dtype=torch.float32, device=self.device)
+            self.backend.set_ant_info(self._ant_params, None, self._ant_origin)
+        self._ant_keys = self.ant.info_keys() if self.ant_info else ((), ())
         if self._np_rngs is None:
             self._np_rngs = self._new_np_rngs([None] * self.num_envs)
         self.init_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)
@@ -275,6 +374,7 @@ class MazeVectorEnv(VectorEnv):
         p, rest, gl, rl = self._device_tables()
         self.backend.reset_maze(mask.to(torch.uint8), rest, p, gl, rl, self._dev_seed, self.env_offset, self._episode, out)
         self._elapsed.masked_fill_(mask, 0)
+        self._set_origin(mask, out)
 
     def _reset_envs(self, mask, out, options=None):
         if self.rng_mode == "device":
@@ -294,10 +394,36 @@ class MazeVectorEnv(VectorEnv):
         st[idx] = rec
         self._elapsed[idx] = 0
         self.backend.refresh(mask.to(torch.uint8), out)
+        self._set_origin(mask, out)
+
+    def _set_origin(self, mask, out):
+        """Ant-v5's init_qpos[:2] <- the reset position of the envs just reset (ant_maze_v5.py:285); set_state leaves it alone."""
+        if self._ant_origin is not None:
+            torch.where(mask[:, None], out["achieved"], self._ant_origin, out=self._ant_origin)
+
+    def _new_ant_rows(self):
+        """Every call that returns info gets its own rows, so that the info of one step stays valid after the next."""
+        if self.ant_info:
+            self._ant_rows = torch.zeros((self.num_envs, len(ANT_INFO_COLUMNS)), dtype=torch.float32, device=self.device)
+            self.backend.set_ant_info(self._ant_params, self._ant_rows, self._ant_origin)
 
     # ------------------------------------------------------------------ gymnasium API
+    # ant_info=True adds the Ant's info (views of the call's [N, 9] rows, each key with its `_key` mask).  Gymnasium's vector
+    # convention: an env reset instead of stepped (NEXT_STEP) reports the reset keys (the refresh of its reset wrote them) and 0 under the
+    # other keys, which its mask marks absent; SAME_STEP puts the finished episodes' keys into final_info.
+    def reset(self, *, seed=None, options=None):
+        self._new_ant_rows()
+        return super().reset(seed=seed, options=options)
+
     def _reset_info(self, out):
-        return {"success": out["success"] > 0}
+        info = {"success": out["success"] > 0}
+        for k, c in self._ant_keys[1]:
+            info[k], info["_" + k] = self._ant_rows[:, c], self._const_true
+        return info
+
+    def _kernel_input(self, actions):
+        self._new_ant_rows()
+        return super()._kernel_input(actions)
 
     def _success(self, column):
         return column > 0
@@ -305,11 +431,31 @@ class MazeVectorEnv(VectorEnv):
     def _step_results(self, out):
         reward, terminated, truncated, info = super()._step_results(out)
         info["success"] = self._success(out["success"])
+        for k, c in self._ant_keys[0]:
+            info[k], info["_" + k] = self._ant_rows[:, c], self._const_true
         return reward, terminated, truncated, info
+
+    def _step_only_masks(self, info, absent):
+        present = ~absent
+        reset_keys = {k for k, _ in self._ant_keys[1]}
+        for k, _ in self._ant_keys[0]:
+            if k not in reset_keys:
+                info["_" + k] = present
 
     def _mask_results(self, out, pre, reward, terminated, truncated, info):
         info["success"] = info["success"] & ~pre
+        if self.ant_info:
+            self._step_only_masks(info, pre)
         return super()._mask_results(out, pre, reward, terminated, truncated, info)
+
+    def _final_info(self, out, info, done):
+        final = super()._final_info(out, info, done)
+        if self.ant_info:
+            rows = self._ant_rows.clone()    # the refresh of the reset below rewrites the finished envs' rows with their reset info
+            for k, c in self._ant_keys[0]:
+                final[k], final["_" + k] = rows[:, c], done
+            self._step_only_masks(info, done)
+        return final
 
     def _after_autoreset(self, out, info):
         # rng_mode="device": the step launch has updated the goals already (the envs it reset got the reset draw after it)

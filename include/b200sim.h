@@ -180,6 +180,25 @@ int b200sim_reset_maze(b200sim_t* h, const unsigned char* mask, const float* res
  * b200sim_refresh and the resets never update the goal. */
 int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
                             int env_offset, const int* episode);
+/* The Ant's keywords and per-step info (AntMaze; reference: ant_maze_v5.py:221-310 forwarding to Gymnasium's Ant-v5 / Ant-v4 [ext]).
+ * Only a handle created with a maze task of touch_mode 2 (no contact forces observed), 3 (cfrc_ext[1:] observed, Ant-v5, (105,)) or 4
+ * (all of cfrc_ext observed, world row first, Ant-v4 use_contact_forces, (111,)) takes it: those handles run the ant kernel build
+ * (csrc/b200sim_ant.cu), any other handle returns an error.  The observed forces are clipped to contact_force_range.  rows: DEVICE
+ * [N, 9] fp32, one row per env: x_position, y_position, distance_from_origin, x_velocity, y_velocity, reward_forward, reward_ctrl,
+ * reward_contact, reward_survive; every b200sim_step writes the rows of all envs, every refresh (the resets included) writes the
+ * masked envs' reset info (v5: x, y = qpos[0:2], distance 0; v4: zeros) with the other columns 0.  origin: DEVICE [N, 2], the reset
+ * positions distance_from_origin is measured from under Ant-v5 (the caller keeps it; needed with rows when version is 5).  Both are
+ * read by every later launch and must outlive them; rows NULL: no info (the keywords still act).  The velocities come from the
+ * torso's position of the last forward pass, which the launches keep in the two state-record words after the goal. */
+typedef struct b200sim_ant_params {
+  int version;                      /* 5 (Ant-v5) or 4 (Ant-v4 info rules) */
+  float forward_reward_weight;      /* v5 only (v4: 1) */
+  float ctrl_cost_weight, contact_cost_weight, healthy_reward;
+  int terminate_when_unhealthy;     /* v4: reward_survive = healthy_reward * (is_healthy or this) */
+  int use_contact_forces;           /* v4: reward_ctrl holds -contact_cost */
+  float healthy_z_range[2], contact_force_range[2];
+} b200sim_ant_params_t;
+int b200sim_set_ant_info(b200sim_t* h, const b200sim_ant_params_t* params, float* rows, const float* origin);
 /* Shadow-Hand manipulation (reference: envs/shadow_dexterous_hand/manipulate.py:154-224 _reset_sim, :226-279 _sample_goal).  The
  * reference's reset is a retry loop, so the draws are two calls: `b200sim_reset_hand_pose` writes rest_record + the drawn object
  * start pose into the masked envs' records (their goal survives) for attempt number `attempt` -- the caller then settles with
