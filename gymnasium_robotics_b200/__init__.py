@@ -17,7 +17,7 @@ ENV_IDS = {"FrankaKitchen-v1": dict(kitchen=True, max_episode_steps=280)}   # __
 for _task in ("FetchReach", "FetchPush", "FetchSlide", "FetchPickAndPlace"):
     for _rt, _suffix in (("sparse", ""), ("dense", "Dense")):
         ENV_IDS[f"{_task}{_suffix}-v4"] = dict(task=_task, reward_type=_rt, max_episode_steps=50)
-# AntMaze: the reference registers v3/v4/v5 x sparse/dense (__init__.py:839-958); v5 (Gymnasium Ant-v5) is mirrored
+# AntMaze: the reference registers v3/v4/v5 x sparse/dense (__init__.py:838-958), all three are mirrored
 for _maze, _steps in (("UMaze", 700), ("Open", 700), ("Open_Diverse_G", 700), ("Open_Diverse_GR", 700), ("Medium", 1000),
                       ("Medium_Diverse_G", 1000), ("Medium_Diverse_GR", 1000), ("Large", 1000), ("Large_Diverse_G", 1000),
                       ("Large_Diverse_GR", 1000)):
@@ -28,6 +28,8 @@ for _maze, _steps in (("UMaze", 700), ("Open", 700), ("Open_Diverse_G", 700), ("
         # -v4 (envs/maze/ant_maze_v4.py) is the same class on Gymnasium's Ant-v4 (use_contact_forces defaults to False there): the
         # same ant.xml, frame_skip and maze_v4 logic with the (27,) observation
         ENV_IDS[f"AntMaze_{_maze}{_suffix}-v4"] = dict(maze=_maze, reward_type=_rt, max_episode_steps=_steps)
+        # -v3 (envs/maze/ant_maze_v3.py) wraps Gymnasium's Ant-v4 too, with the older task logic of envs/maze/maze.py (maze_version=3)
+        ENV_IDS[f"AntMaze_{_maze}{_suffix}-v3"] = dict(maze=_maze, reward_type=_rt, max_episode_steps=_steps, maze_version=3)
 # PointMaze-v3 (__init__.py:960-1080)
 for _maze, _steps in (("UMaze", 300), ("Open", 300), ("Open_Diverse_G", 300), ("Open_Diverse_GR", 300), ("Medium", 600),
                       ("Medium_Diverse_G", 600), ("Medium_Diverse_GR", 600), ("Large", 800), ("Large_Diverse_G", 800),
@@ -57,6 +59,11 @@ for _rt, _suffix in (("dense", ""), ("sparse", "Sparse")):
     ENV_IDS[f"AdroitHandPen{_suffix}-v2"] = dict(adroit_task="AdroitHandPen", reward_type=_rt, max_episode_steps=200)
 
 
+def _ant_version(env_id):
+    """The Ant an AntMaze id wraps: Ant-v5 (-v5), Ant-v4 (-v4 and -v3, ant_maze_v3.py:7)."""
+    return 4 if env_id.endswith("-v3") else int(env_id[-1])
+
+
 def make_vec(env_id: str, num_envs: int = 1, **kwargs):
     """Batched replacement for `gym.make_vec(env_id, num_envs=...)` (reference ids, e.g. "FetchPickAndPlace-v4")."""
     if env_id.startswith("FrankaKitchen"):
@@ -73,7 +80,7 @@ def make_vec(env_id: str, num_envs: int = 1, **kwargs):
     spec = dict(ENV_IDS[env_id])
     spec.update(kwargs)
     if env_id.startswith("AntMaze_"):
-        spec["ant_version"] = int(env_id[-1])   # the Ant the id wraps: Ant-v5 (-v5) or Ant-v4 (-v4)
+        spec["ant_version"] = _ant_version(env_id)
     if "maze" in spec:
         from .maze import MazeVectorEnv
 
@@ -118,6 +125,6 @@ def register_envs():
         if "adroit_task" in kw:
             kw["task"] = kw.pop("adroit_task")
         if env_id.startswith("AntMaze_"):
-            kw["ant_version"] = int(env_id[-1])
+            kw["ant_version"] = _ant_version(env_id)
         register(id=env_id, vector_entry_point=ep, kwargs=kw)
     return True

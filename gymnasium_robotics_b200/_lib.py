@@ -46,7 +46,8 @@ class UniformResetC(ctypes.Structure):
 
 class MazeResetC(ctypes.Structure):
     """b200sim_maze_reset_t"""
-    _fields_ = [("n_goal", ctypes.c_int), ("n_reset", ctypes.c_int), ("scaling", ctypes.c_float), ("noise", ctypes.c_float)]
+    _fields_ = [("n_goal", ctypes.c_int), ("n_reset", ctypes.c_int), ("scaling", ctypes.c_float), ("noise", ctypes.c_float),
+                ("separation", ctypes.c_float)]
 
 
 class HandResetC(ctypes.Structure):
@@ -134,6 +135,7 @@ def lib():
     L.b200sim_reset_uniform.argtypes = [vp, vp, vp, ctypes.POINTER(UniformResetC), ctypes.c_ulonglong, ci, vp] + [vp] * 6
     L.b200sim_set_obs_noise.argtypes = [vp, vp, ctypes.c_ulonglong, ci, vp]
     L.b200sim_set_goal_update.argtypes = [vp, vp, ci, ctypes.c_float, ctypes.c_float, ctypes.c_ulonglong, ci, vp]
+    L.b200sim_set_goal_redraw.argtypes = [vp, vp, ci, ctypes.c_float, ctypes.c_float, ctypes.c_ulonglong, ci, vp]
     L.b200sim_set_ant_info.argtypes = [vp, ctypes.POINTER(AntParamsC), vp, vp]
     L.b200sim_launch_count.argtypes = [vp]
     L.b200sim_launch_count.restype = ctypes.c_long
@@ -143,6 +145,6 @@ def lib():
 
 
 EXPORTED_SYMBOLS = ["b200sim_create", "b200sim_destroy", "b200sim_last_error", "b200sim_num_envs", "b200sim_layout",
-                    "b200sim_state", "b200sim_step", "b200sim_refresh", "b200sim_raw_step", "b200sim_raw_step_masked", "b200sim_compute_reward", "b200sim_reset", "b200sim_reset_uniform", "b200sim_reset_maze", "b200sim_check_state", "b200sim_reset_reach", "b200sim_reset_hand_pose", "b200sim_reset_hand_goal", "b200sim_set_obs_noise", "b200sim_set_goal_update", "b200sim_set_ant_info",
+                    "b200sim_state", "b200sim_step", "b200sim_refresh", "b200sim_raw_step", "b200sim_raw_step_masked", "b200sim_compute_reward", "b200sim_reset", "b200sim_reset_uniform", "b200sim_reset_maze", "b200sim_check_state", "b200sim_reset_reach", "b200sim_reset_hand_pose", "b200sim_reset_hand_goal", "b200sim_set_obs_noise", "b200sim_set_goal_update", "b200sim_set_goal_redraw", "b200sim_set_ant_info",
                     "b200sim_launch_count", "b200sim_launch_config", "b200sim_set_time_limit", "b200sim_elapsed", "b200sim_overflow_counter",
                     "b200sim_packed_width", "b200sim_set_packed"]

@@ -100,6 +100,22 @@ __global__ void maze_goal_update_kernel(GoalUpdateArgs g, float radius, int N, i
     rec[st_goal] = goal[0]; rec[st_goal + 1] = goal[1];
   }
 }
+// b200sim_set_goal_redraw (AntMaze-v3): the same thread layout and key; one candidate, and the env's reward in the step's outputs
+// (reward[i * reward_stride]: the separate buffer or the packed column) is written again against the new goal
+__global__ void maze_goal_redraw_kernel(GoalUpdateArgs g, float radius, int dense, int N, int stride, int st_qpos, int st_goal,
+                                        float* __restrict__ state, const int* __restrict__ elapsed, float* __restrict__ reward,
+                                        int reward_stride) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  float* rec = state + (size_t)i * stride;
+  const float ach[2] = {rec[st_qpos], rec[st_qpos + 1]};
+  float goal[2] = {rec[st_goal], rec[st_goal + 1]}, r;
+  if (rs_maze_goal_redraw(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, dense, g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
+                          (uint32_t)elapsed[i], ach, goal, &r)) {
+    rec[st_goal] = goal[0]; rec[st_goal + 1] = goal[1];
+    reward[(size_t)i * reward_stride] = r;
+  }
+}
 
 __global__ void check_state_kernel(int N, int stride, float* __restrict__ state, const float* __restrict__ rest, b200sim_keep_t keep,
                                    unsigned char* __restrict__ bad) {
@@ -168,7 +184,8 @@ struct b200sim {
   int max_steps = 0, term_on_success = 0;        // b200sim_set_time_limit
   int packed = 0, packed_w = 0;                  // b200sim_set_packed
   ObsNoiseArgs noise = {nullptr, nullptr, 0, 0};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
-  GoalUpdateArgs goal_update = {nullptr, 0, 0.f, 0.f, 0, 0, nullptr};   // b200sim_set_goal_update (maze tasks)
+  GoalUpdateArgs goal_update = {nullptr, 0, 0.f, 0.f, 0, 0, nullptr};   // b200sim_set_goal_update / b200sim_set_goal_redraw (maze tasks)
+  int goal_redraw = 0;                                                  // 1: the slot above is b200sim_set_goal_redraw's
   // b200sim_set_ant_info (ant build): Ant-v5's defaults, no info rows until set
   AntInfoArgs ant = {-1.f, 1.f, 1.f, 0.5f, 5e-4f, 1.f, 0.2f, 1.f, 0, 0, 0, nullptr, nullptr};
   size_t smem_bytes = 0;
@@ -428,20 +445,37 @@ int b200sim_step(b200sim_t* h, const float* actions, float* obs, float* achieved
   const int rc = launch(h, MODE_STEP, 0, actions, nullptr, obs, achieved, desired, reward, success, terminated, truncated, info, stream);
   if (rc != 0 || !h->goal_update.goal_xy) return rc;
   ON_DEVICE(h);
-  maze_goal_update_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->task.success_radius, h->N, h->task.st_stride,
-                                                                               h->task.st_qpos, h->task.st_goal, h->state, h->elapsed);
+  const FetchTask& t = h->task;
+  if (h->goal_redraw) {
+    float* rew = h->packed ? obs + t.nobs + 2 * t.ngoal : reward;   // the reward column of the packed row (launch) or the buffer
+    maze_goal_redraw_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, t.success_radius, t.reward_dense, h->N,
+                                                                                 t.st_stride, t.st_qpos, t.st_goal, h->state, h->elapsed, rew,
+                                                                                 h->packed ? h->packed_w : 1);
+  } else {
+    maze_goal_update_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->task.success_radius, h->N, h->task.st_stride,
+                                                                                 h->task.st_qpos, h->task.st_goal, h->state, h->elapsed);
+  }
   h->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
 }
+static int set_goal_slot(b200sim* h, const char* fn, int redraw, const float* goal_xy, int n_goal, float scaling, float noise,
+                         unsigned long long seed, int env_offset, const int* episode) {
+  if (h->task.kind != TASK_ANTMAZE) return fail(h, std::string(fn) + ": not a maze task", -6);
+  if (goal_xy && !episode) return fail(h, std::string(fn) + ": episode is NULL", -1);
+  if (goal_xy && n_goal < 2) return fail(h, std::string(fn) + ": fewer than two goal cells", -1);
+  if (env_offset < 0) return fail(h, std::string(fn) + ": negative env_offset", -1);
+  h->goal_update = goal_xy ? GoalUpdateArgs{goal_xy, n_goal, scaling, noise, seed, env_offset, episode} : GoalUpdateArgs{nullptr, 0, 0.f, 0.f, 0, 0, nullptr};
+  h->goal_redraw = goal_xy && redraw ? 1 : 0;
+  return 0;
+}
 int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
                             int env_offset, const int* episode) {
-  if (h->task.kind != TASK_ANTMAZE) return fail(h, "b200sim_set_goal_update: not a maze task", -6);
-  if (goal_xy && !episode) return fail(h, "b200sim_set_goal_update: episode is NULL", -1);
-  if (goal_xy && n_goal < 2) return fail(h, "b200sim_set_goal_update: fewer than two goal cells", -1);
-  if (env_offset < 0) return fail(h, "b200sim_set_goal_update: negative env_offset", -1);
-  h->goal_update = goal_xy ? GoalUpdateArgs{goal_xy, n_goal, scaling, noise, seed, env_offset, episode} : GoalUpdateArgs{nullptr, 0, 0.f, 0.f, 0, 0, nullptr};
-  return 0;
+  return set_goal_slot(h, "b200sim_set_goal_update", 0, goal_xy, n_goal, scaling, noise, seed, env_offset, episode);
+}
+int b200sim_set_goal_redraw(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
+                            int env_offset, const int* episode) {
+  return set_goal_slot(h, "b200sim_set_goal_redraw", 1, goal_xy, n_goal, scaling, noise, seed, env_offset, episode);
 }
 int b200sim_set_ant_info(b200sim_t* h, const b200sim_ant_params_t* p, float* rows, const float* origin) {
   if (h->unit != &kernel_unit_ant) return fail(h, "b200sim_set_ant_info: not an ant-build handle (maze task with touch_mode 2..4)", -6);

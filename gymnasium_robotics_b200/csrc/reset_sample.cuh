@@ -112,7 +112,8 @@ RS_HD void rs_uniform_reset_record(const b200sim_uniform_reset_t& p, unsigned lo
 }
 
 // Maze reset (envs/maze/maze_v4.py:299-358 MazeEnv.reset with generate_target_goal :256-274, generate_reset_pos :276-297,
-// add_xy_position_noise :360-373): goal = a goal cell + noise, start = a reset cell farther than half a cell from the goal + noise.
+// add_xy_position_noise :360-373): goal = a goal cell + noise, start = a reset cell farther than `p.separation` from the goal + noise
+// (0: half a cell, 0.5 * scaling; AntMaze-v3's envs/maze/maze.py:194 uses 0.5).
 // `goal_xy` / `reset_xy` are the cell-centre tables ([n, 2]); an index is (word * n) >> 32 (bias < n / 2^32).
 #define RS_MAZE_POS_BLOCKS 32   // 128 candidate reset cells at most
 RS_HD void rs_maze_reset_draw(const b200sim_maze_reset_t& p, const float* goal_xy, const float* reset_xy, unsigned long long seed, uint32_t env,
@@ -120,6 +121,7 @@ RS_HD void rs_maze_reset_draw(const b200sim_maze_reset_t& p, const float* goal_x
   const uint32_t key[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
   uint32_t ctr[4] = {env, episode, 0u, 0x3A2Eu}, r[4];
   const float amp = p.noise * p.scaling;
+  const float sep = p.separation > 0.f ? p.separation : 0.5f * p.scaling;
   rs_philox4x32_10(ctr, key, r);
   uint32_t gi = (uint32_t)(((uint64_t)r[0] * (uint64_t)p.n_goal) >> 32);
   goal[0] = goal_xy[2 * gi] + (2.0f * rs_u01(r[1]) - 1.0f) * amp;
@@ -133,7 +135,7 @@ RS_HD void rs_maze_reset_draw(const b200sim_maze_reset_t& p, const float* goal_x
       uint32_t ri = (uint32_t)(((uint64_t)r[h] * (uint64_t)p.n_reset) >> 32);
       pos[0] = reset_xy[2 * ri]; pos[1] = reset_xy[2 * ri + 1];
       float dx = pos[0] - goal[0], dy = pos[1] - goal[1];
-      done = !(sqrtf(dx * dx + dy * dy) <= 0.5f * p.scaling);     // maze_v4.py:289-296
+      done = !(sqrtf(dx * dx + dy * dy) <= sep);     // maze_v4.py:289-296, maze.py:193-198
     }
   }
   ctr[2] = RS_MAZE_POS_BLOCKS + 1;
@@ -163,13 +165,15 @@ RS_HD float rs_maze_goal_distance(const float ach[2], const float goal[2]) {
   return sqrtf(dx * dx + dy * dy);
 #endif
 }
+// MAX_CANDIDATES 1 is AntMaze-v3's single draw (rs_maze_goal_redraw below).
+template <int MAX_CANDIDATES = RS_MAZE_GOAL_CANDIDATES>
 RS_HD int rs_maze_goal_update(const float* goal_xy, int n_goal, float scaling, float noise, float radius, unsigned long long seed,
                               uint32_t env, uint32_t episode, uint32_t step, const float ach[2], float goal[2]) {
   if (!(rs_maze_goal_distance(ach, goal) <= radius)) return 0;
   const uint32_t key[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
   const float amp = noise * scaling;
   int c = 0;
-  while (c < RS_MAZE_GOAL_CANDIDATES) {
+  while (c < MAX_CANDIDATES) {
     uint32_t ctr[4] = {env, episode, step, RS_MAZE_GOAL_TAG | ((uint32_t)c << 16)}, r[4];
     rs_philox4x32_10(ctr, key, r);
     c++;
@@ -185,6 +189,19 @@ RS_HD int rs_maze_goal_update(const float* goal_xy, int n_goal, float scaling, f
     if (!(rs_maze_goal_distance(ach, goal) <= radius)) break;
   }
   return c;
+}
+
+// Goal redraw of a continuing AntMaze-v3 task (envs/maze/maze.py:283-302: compute_terminated draws generate_target_goal +
+// add_xy_position_noise once, with no rejection, for an env within the radius of its goal).  The draw is candidate 0 of
+// rs_maze_goal_update and is kept even when it lands within the radius.  ant_maze_v3.py:94-97 computes the reward after that, so
+// `reward` is the step's reward against the new goal: reward_kernel's formula (b200sim.cu) on rs_maze_goal_distance, which rounds as
+// reward_kernel does, so the two agree bit for bit.  Returns 1 when the goal changed (`goal` and `reward` written), 0 otherwise.
+RS_HD int rs_maze_goal_redraw(const float* goal_xy, int n_goal, float scaling, float noise, float radius, int dense, unsigned long long seed,
+                              uint32_t env, uint32_t episode, uint32_t step, const float ach[2], float goal[2], float* reward) {
+  if (!rs_maze_goal_update<1>(goal_xy, n_goal, scaling, noise, radius, seed, env, episode, step, ach, goal)) return 0;
+  const float d = rs_maze_goal_distance(ach, goal);
+  *reward = dense ? expf(-d) : (d <= radius ? 1.f : 0.f);
+  return 1;
 }
 
 RS_HD void rs_maze_reset_record(const b200sim_maze_reset_t& p, const float* goal_xy, const float* reset_xy, unsigned long long seed, uint32_t env,

@@ -192,16 +192,20 @@ class CudaBackend:
         self._check(self.L.b200sim_set_obs_noise(self.h, scale.data_ptr() if scale is not None else None, int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                  int(env_offset), episode.data_ptr() if scale is not None else None))
 
-    def set_goal_update(self, goal_xy, scaling, noise, seed, env_offset, episode):
+    def set_goal_update(self, goal_xy, scaling, noise, seed, env_offset, episode, fn="b200sim_set_goal_update"):
         """b200sim_set_goal_update (maze tasks): every later step redraws the goal of the envs that succeeded, per (seed, env,
         episode, step); goal_xy None turns the update off.  The handle keeps both pointers: the tensors must outlive its steps."""
         if goal_xy is not None:
             assert goal_xy.is_cuda and goal_xy.dtype == torch.float32 and goal_xy.is_contiguous() and goal_xy.dim() == 2 and goal_xy.shape[1] == 2
             assert episode.is_cuda and episode.dtype == torch.int32 and episode.is_contiguous() and episode.numel() == self.num_envs
         on = goal_xy is not None
-        self._check(self.L.b200sim_set_goal_update(self.h, goal_xy.data_ptr() if on else None, len(goal_xy) if on else 0, float(scaling),
-                                                   float(noise), int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset),
-                                                   episode.data_ptr() if on else None))
+        self._check(getattr(self.L, fn)(self.h, goal_xy.data_ptr() if on else None, len(goal_xy) if on else 0, float(scaling),
+                                        float(noise), int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset), episode.data_ptr() if on else None))
+
+    def set_goal_redraw(self, goal_xy, scaling, noise, seed, env_offset, episode):
+        """b200sim_set_goal_redraw (AntMaze-v3): every later step draws ONE new goal for the envs that succeeded and writes their
+        reward again against it; it shares the handle's slot with set_goal_update (setting one replaces the other)."""
+        self.set_goal_update(goal_xy, scaling, noise, seed, env_offset, episode, fn="b200sim_set_goal_redraw")
 
     def set_ant_info(self, params, rows, origin):
         """b200sim_set_ant_info (ant-build handles): the Ant's keywords, and the [N, 9] info rows later launches write (None: no rows)

@@ -63,9 +63,11 @@ def model_name(agent, maze):
 
 
 class MazeCells:
-    """Cell bookkeeping of `Maze` (maze_v4.py:26-242) without the XML part."""
+    """Cell bookkeeping of `Maze` (maze_v4.py:26-242) without the XML part.  fallbacks=False is the older `Maze` of AntMaze-v3
+    (envs/maze/maze.py:86-157): a layout with no "r"/"c" cells gets no reset locations and one with no "g"/"c" cells no goal locations
+    (maze_v4.py:223-230 would take the empty cells); an unlabelled layout still uses every free cell for both."""
 
-    def __init__(self, maze_map, scaling=SCALING):
+    def __init__(self, maze_map, scaling=SCALING, fallbacks=True):
         self.maze_map, self.scaling = maze_map, scaling
         self.length, self.width = len(maze_map), len(maze_map[0])
         self.x_center, self.y_center = self.width / 2 * scaling, self.length / 2 * scaling
@@ -83,9 +85,9 @@ class MazeCells:
                     empty.append(xy)
         if not goals and not resets and not combined:
             combined = empty
-        elif not resets and not combined:
+        elif fallbacks and not resets and not combined:
             resets = empty
-        elif not goals and not combined:
+        elif fallbacks and not goals and not combined:
             goals = empty
         self.goal_locations = np.array(goals + combined)
         self.reset_locations = np.array(resets + combined)
@@ -97,8 +99,9 @@ class MazeCells:
         return np.array([math.floor((self.y_center - xy[1]) / self.scaling), math.floor((xy[0] + self.x_center) / self.scaling)])
 
 
-def check_maze_map(maze_map, scaling):
-    """The cells of a user layout (`maze_map=`) as a list of rows, or ValueError with the reason.  Beyond the reference, a
+def check_maze_map(maze_map, scaling, fallbacks=True):
+    """The cells of a user layout (`maze_map=`) as a list of rows, or ValueError with the reason.  fallbacks=False (AntMaze-v3,
+    `MazeCells`) refuses a layout that labels cells but leaves no goal or no reset location.  Beyond the reference, a
     layout is refused when some goal location has no reset location in another cell: the reference's start draw
     (`generate_reset_pos`, maze_v4.py:276-297) would loop forever on it, and the device draw (csrc/reset_sample.cuh) would give up and start the env
     in its goal cell."""
@@ -115,7 +118,7 @@ def check_maze_map(maze_map, scaling):
             if not (cell in (R, G, C) if isinstance(cell, str) else
                     (isinstance(cell, (int, np.integer)) and not isinstance(cell, bool) and cell in (0, 1))):
                 raise ValueError(f"maze_map[{i}][{j}] = {cell!r}: a cell is 0, 1, {R!r}, {G!r} or {C!r}")
-    cells = MazeCells(rows, scaling)
+    cells = MazeCells(rows, scaling, fallbacks)
     if len(cells.goal_locations) == 0 or len(cells.reset_locations) == 0:
         raise ValueError(f"maze_map has no {'goal' if len(cells.goal_locations) == 0 else 'reset'} location")
     for g in cells.goal_locations:
@@ -231,7 +234,13 @@ class MazeVectorEnv(VectorEnv):
     0, 1, "r", "g", "c" cells (`check_maze_map`), built on the agent's committed model (`models.build_maze_model`) unless a
     `model` is given; the named `maze` still supplies the episode length.  The per-env numpy streams exist in every rng_mode:
     explicit `options` cells draw from them, and so does the goal update of `reset_target` except in rng_mode="device", where
-    the step launch redraws the goals of the envs that succeeded (b200sim_set_goal_update)."""
+    the step launch redraws the goals of the envs that succeeded (b200sim_set_goal_update).
+
+    maze_version=3 (ant agent only) is AntMaze-v3's task logic, envs/maze/maze.py on Gymnasium's Ant-v4 (ant_maze_v3.py): the start
+    is drawn farther than 0.5 (not half a cell) from the goal, a labelled layout gets no empty-cell fallbacks, `reset_target` does not
+    exist, and in a continuing task with more than one goal location an env that reaches its goal gets one new goal inside the step
+    (maze.py:283-302) whose reward is that of the new goal (ant_maze_v3.py:94-97).  The step's info is the Ant's (`ant_info` defaults
+    to True) with no `success` key, and the reset info is empty."""
 
     metadata = {"render_modes": [], "render_fps": 50, "autoreset_mode": "next_step"}
     AGENT = "ant"
@@ -239,17 +248,31 @@ class MazeVectorEnv(VectorEnv):
     SUCCESS_KEY = "success"
 
     def __init__(self, maze="Large", num_envs: int = 1, reward_type: str = "sparse", continuing_task: bool = True,
-                 reset_target: bool = False, max_episode_steps: Optional[int] = None, device="cuda:0", rng_mode: str = "auto",
+                 reset_target: Optional[bool] = None, max_episode_steps: Optional[int] = None, device="cuda:0", rng_mode: str = "auto",
                  autoreset_mode: str = "next_step", backend_factory=None, agent: Optional[str] = None, model=None,
                  include_cfrc_ext_in_observation: Optional[bool] = None, maze_map=None, ant_version: Optional[int] = None,
-                 ant_info: bool = False, **kwargs):
+                 ant_info: Optional[bool] = None, maze_version: int = 4, **kwargs):
         self.agent = agent or self.AGENT
         cfg = AGENTS[self.agent]
-        # the Ant's keywords (Gymnasium's Ant-v5 for the -v5 ids and by default, Ant-v4 for the -v4 ids); they leave `kwargs`
+        if maze_version not in (3, 4):
+            raise ValueError(f"maze_version must be 3 or 4, got {maze_version!r}")
+        v3 = self._v3 = maze_version == 3
+        self.maze_version = maze_version
+        if v3:
+            if self.agent != "ant":
+                raise ValueError("maze_version=3 (envs/maze/maze.py) is AntMaze-v3's; PointMaze-v3 runs the maze_v4 logic (maze_version=4)")
+            if ant_version not in (None, 4):
+                raise ValueError(f"AntMaze-v3 wraps Ant-v4, got ant_version={ant_version!r}")
+            if reset_target is not None:   # v3's MazeEnv takes it into **kwargs and forwards it to Ant-v4, which refuses it
+                raise TypeError("AntEnv.__init__() got an unexpected keyword argument 'reset_target'")
+            ant_version = 4
+        # the Ant's keywords (Gymnasium's Ant-v5 for the -v5 ids and by default, Ant-v4 for the -v4 and -v3 ids); they leave `kwargs`
         self.ant = AntKeywords(5 if ant_version is None else ant_version, kwargs, include_cfrc_ext_in_observation) if self.agent == "ant" else None
         if self.ant is None and (ant_info or ant_version is not None):
             raise ValueError("ant_version / ant_info are keywords of the ant agent")
-        self.ant_info = bool(ant_info)
+        # AntMaze-v3's step info IS Ant-v4's (ant_maze_v3.py:91), so it is on by default there
+        self.ant_info = v3 if ant_info is None else bool(ant_info)
+        reset_target = bool(reset_target)
         if isinstance(maze, str) and maze not in MAPS:
             raise KeyError(f"unknown maze {maze!r}")
         if reward_type not in ("sparse", "dense"):
@@ -261,10 +284,12 @@ class MazeVectorEnv(VectorEnv):
         if maze_map is not None:
             if not named:
                 raise ValueError("give the layout once: as `maze_map=` or as an explicit `maze` cell list, not both")
-            layout = check_maze_map(maze_map, cfg["scaling"])
+            layout = check_maze_map(maze_map, cfg["scaling"], fallbacks=not v3)
         else:
             layout = MAPS[maze] if named else maze
-        self.cells = MazeCells(layout, cfg["scaling"])
+        self.cells = MazeCells(layout, cfg["scaling"], fallbacks=not v3)
+        # generate_reset_pos draws the start again while it lies within this distance of the goal (maze_v4.py:290; maze.py:194)
+        self.separation = 0.5 if v3 else 0.5 * cfg["scaling"]
         if model is None and not named:
             raise ValueError("an explicit maze map needs its compiled `model` (see models.compile_maze_model)")
         if model is not None:
@@ -306,9 +331,14 @@ class MazeVectorEnv(VectorEnv):
         # update_goal (maze_v4.py:400-418) acts only in a continuing task with reset_target and more than one goal location; in
         # rng_mode="device" the step launch does it (b200sim_set_goal_update), keyed by the seed the library was last given
         self._goal_update_on = continuing_task and reset_target and len(self.cells.goal_locations) > 1
+        # AntMaze-v3's redraw (maze.py:283-302) acts in a continuing task with more than one goal location; in rng_mode="device" the
+        # step launch does it (b200sim_set_goal_redraw), rewriting the reward too
+        self._goal_redraw_on = v3 and continuing_task and len(self.cells.goal_locations) > 1
         self._goal_update_seed = None
         if self.rng_mode == "device" and self._goal_update_on and not hasattr(self.backend, "set_goal_update"):
             raise NotImplementedError(f"{type(self.backend).__name__} cannot update goals on the device (no set_goal_update)")
+        if self.rng_mode == "device" and self._goal_redraw_on and not hasattr(self.backend, "set_goal_redraw"):
+            raise NotImplementedError(f"{type(self.backend).__name__} cannot redraw goals on the device (no set_goal_redraw)")
 
     # ------------------------------------------------------------------ sampling (MazeEnv.reset, maze_v4.py:299-358)
     def _noise_np(self, rng, xy):
@@ -332,7 +362,7 @@ class MazeVectorEnv(VectorEnv):
             pos = cells.cell_rowcol_to_xy(rc)
         else:
             pos = goal.copy()
-            while np.linalg.norm(pos - goal) <= 0.5 * self.scaling:
+            while np.linalg.norm(pos - goal) <= self.separation:
                 pos = cells.reset_locations[rng.integers(low=0, high=len(cells.reset_locations))].copy()
         return goal, self._noise_np(rng, pos)
 
@@ -346,10 +376,10 @@ class MazeVectorEnv(VectorEnv):
         ri = lambda hi, k: torch.randint(0, hi, (k,), generator=self._gen, device=self.device)
         goal = self._goal_loc[ri(len(self._goal_loc), n)] + (u(n, 2) * 2 - 1) * NOISE * self.scaling
         pos = self._reset_loc[ri(len(self._reset_loc), n)]
-        bad = torch.linalg.norm(pos - goal, dim=1) <= 0.5 * self.scaling
+        bad = torch.linalg.norm(pos - goal, dim=1) <= self.separation
         while bool(bad.any()):
             pos[bad] = self._reset_loc[ri(len(self._reset_loc), int(bad.sum()))]
-            bad = torch.linalg.norm(pos - goal, dim=1) <= 0.5 * self.scaling
+            bad = torch.linalg.norm(pos - goal, dim=1) <= self.separation
         return goal, pos + (u(n, 2) * 2 - 1) * NOISE * self.scaling
 
     def _rest_record(self):   # ant_env.init_qpos, zero velocities
@@ -363,10 +393,12 @@ class MazeVectorEnv(VectorEnv):
 
             p = MazeResetC()
             p.n_goal, p.n_reset, p.scaling, p.noise = len(self._goal_loc), len(self._reset_loc), float(self.scaling), float(NOISE)
+            p.separation = self.separation if self._v3 else 0.0   # 0: the library's half cell, bit for bit the v4 draw
             self._dev_reset = (p, self._rest, self._goal_loc.contiguous(), self._reset_loc.contiguous())
             self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
-        if self._goal_update_on and self._goal_update_seed != self._dev_seed:   # first reset, or reset(seed=...) gave a new key
-            self.backend.set_goal_update(self._dev_reset[2], self.scaling, NOISE, self._dev_seed, self.env_offset, self._episode)
+        if (self._goal_update_on or self._goal_redraw_on) and self._goal_update_seed != self._dev_seed:   # first reset, or a new key
+            setter = self.backend.set_goal_redraw if self._goal_redraw_on else self.backend.set_goal_update
+            setter(self._dev_reset[2], self.scaling, NOISE, self._dev_seed, self.env_offset, self._episode)
             self._goal_update_seed = self._dev_seed
         return self._dev_reset
 
@@ -416,7 +448,7 @@ class MazeVectorEnv(VectorEnv):
         return super().reset(seed=seed, options=options)
 
     def _reset_info(self, out):
-        info = {"success": out["success"] > 0}
+        info = {} if self._v3 else {"success": out["success"] > 0}   # v3: Ant-v4's reset info, {}
         for k, c in self._ant_keys[1]:
             info[k], info["_" + k] = self._ant_rows[:, c], self._const_true
         return info
@@ -430,7 +462,8 @@ class MazeVectorEnv(VectorEnv):
 
     def _step_results(self, out):
         reward, terminated, truncated, info = super()._step_results(out)
-        info["success"] = self._success(out["success"])
+        if not self._v3:   # v3's step info is the Ant's alone (ant_maze_v3.py:91)
+            info["success"] = self._success(out["success"])
         for k, c in self._ant_keys[0]:
             info[k], info["_" + k] = self._ant_rows[:, c], self._const_true
         return reward, terminated, truncated, info
@@ -443,13 +476,14 @@ class MazeVectorEnv(VectorEnv):
                 info["_" + k] = present
 
     def _mask_results(self, out, pre, reward, terminated, truncated, info):
-        info["success"] = info["success"] & ~pre
+        if "success" in info:
+            info["success"] = info["success"] & ~pre
         if self.ant_info:
             self._step_only_masks(info, pre)
         return super()._mask_results(out, pre, reward, terminated, truncated, info)
 
     def _final_info(self, out, info, done):
-        final = super()._final_info(out, info, done)
+        final = {} if self._v3 else super()._final_info(out, info, done)
         if self.ant_info:
             rows = self._ant_rows.clone()    # the refresh of the reset below rewrites the finished envs' rows with their reset info
             for k, c in self._ant_keys[0]:
@@ -461,6 +495,8 @@ class MazeVectorEnv(VectorEnv):
         # rng_mode="device": the step launch has updated the goals already (the envs it reset got the reset draw after it)
         if self._goal_update_on and self.rng_mode != "device":
             self._update_goal(info["success"], out)  # maze_v4.py:400-418 (never for the envs that were just reset: `success` is masked)
+        if self._goal_redraw_on and self.rng_mode != "device":
+            self._redraw_goal(out)                   # maze.py:283-302 (the success column of the envs just reset is masked to 0)
 
     def _finish_info(self, out, info):
         pass   # `success` as of the step, before a SAME_STEP reset; no mask entry
@@ -481,10 +517,34 @@ class MazeVectorEnv(VectorEnv):
             new[k] = goal
         st[idx, sl["goal"].start:sl["goal"].stop] = torch.as_tensor(new, dtype=torch.float32, device=self.device)
 
+    def _redraw_goal(self, out):
+        """AntMaze-v3's redraw on the host: each succeeding env gets one goal cell + noise, and its reward in the packed row becomes
+        compute_reward against it (ant_maze_v3.py:94-97).  numpy mode: one draw from each succeeding env's stream in the reference's
+        order (`integers`, then two `uniform`s).  torch mode: one candidate for every env from the device generator, applied where
+        the success column is 1, with no host synchronisation."""
+        st, sl, success = self.backend.state, self._sl["goal"], out["success"] > 0
+        if self.rng_mode == "numpy":
+            idx = torch.nonzero(success, as_tuple=False).flatten()
+            if idx.numel() == 0:
+                return
+            cells = self.cells.goal_locations
+            new = np.array([self._noise_np(self._np_rngs[i], cells[self._np_rngs[i].integers(low=0, high=len(cells))].copy())
+                            for i in idx.tolist()])
+            new = torch.as_tensor(new, dtype=torch.float32, device=self.device)
+            st[idx, sl.start:sl.stop] = new
+            out["reward"][idx] = self.backend.compute_reward(out["achieved"][idx], new)
+            return
+        n = self.num_envs
+        gi = torch.randint(0, len(self._goal_loc), (n,), generator=self._gen, device=self.device)
+        new = self._goal_loc[gi] + (torch.rand(n, 2, generator=self._gen, device=self.device) * 2 - 1) * NOISE * self.scaling
+        st[:, sl] = torch.where(success[:, None], new, st[:, sl])
+        out["reward"].copy_(torch.where(success, self.backend.compute_reward(out["achieved"], new), out["reward"]))
+
     def _reward_np_dtype(self):
         return np.float64
 
     def compute_terminated(self, achieved_goal, desired_goal, info=None):
+        # pure in every version: AntMaze-v3's redraw of self.goal inside compute_terminated (maze.py:289-302) happens in step
         if not self.continuing_task:
             return bool(np.linalg.norm(np.asarray(achieved_goal) - np.asarray(desired_goal)) <= SUCCESS_RADIUS)
         return False

@@ -165,6 +165,9 @@ int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long s
 typedef struct b200sim_maze_reset {
   int n_goal, n_reset;
   float scaling, noise;   /* maze_size_scaling; position_noise_range (0.25) */
+  /* the start is drawn again while it lies within `separation` of the goal; 0 means 0.5 * scaling, half a cell (maze_v4.py:290).
+   * AntMaze-v3 (envs/maze/maze.py:194) uses 0.5 at every scaling. */
+  float separation;
 } b200sim_maze_reset_t;
 int b200sim_reset_maze(b200sim_t* h, const unsigned char* mask, const float* rest_record, const b200sim_maze_reset_t* params,
                        const float* goal_xy, const float* reset_xy, unsigned long long seed, int env_offset, int* episode, float* obs,
@@ -179,6 +182,15 @@ int b200sim_reset_maze(b200sim_t* h, const unsigned char* mask, const float* res
  * increments) are read by every later step and must outlive them.  goal_xy NULL: update off.  b200sim_raw_step*,
  * b200sim_refresh and the resets never update the goal. */
 int b200sim_set_goal_update(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
+                            int env_offset, const int* episode);
+/* Goal redraw of a continuing AntMaze-v3 task (reference: envs/maze/maze.py:283-302 compute_terminated, called before compute_reward
+ * in ant_maze_v3.py:94-97).  The arguments and refusals are those of b200sim_set_goal_update, and the two share one slot: setting
+ * either replaces the other, goal_xy NULL turns both off.  From the next b200sim_step on, a small kernel runs after the step kernel:
+ * an env whose success column is 1 gets exactly ONE new goal, candidate 0 of b200sim_set_goal_update's draw (counter (env index +
+ * env_offset, episode[i], step after the step, 0x60A1)), kept even when it lands within success_radius.  The kernel then writes that
+ * env's reward in the step's outputs again, against the new goal (dense exp(-d), sparse d <= success_radius; equal to
+ * b200sim_compute_reward bit for bit).  desired, success and the flags keep the old goal's values. */
+int b200sim_set_goal_redraw(b200sim_t* h, const float* goal_xy, int n_goal, float scaling, float noise, unsigned long long seed,
                             int env_offset, const int* episode);
 /* The Ant's keywords and per-step info (AntMaze; reference: ant_maze_v5.py:221-310 forwarding to Gymnasium's Ant-v5 / Ant-v4 [ext]).
  * Only a handle created with a maze task of touch_mode 2 (no contact forces observed), 3 (cfrc_ext[1:] observed, Ant-v5, (105,)) or 4
