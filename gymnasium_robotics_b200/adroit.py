@@ -24,12 +24,11 @@ import torch
 
 from . import rotations
 from ._lib import FetchTaskC
-from .fetch import CudaBackend
+from .fetch import ADROIT_REF_POINT, CudaBackend  # noqa: F401  (ADROIT_REF_POINT: re-exported)
 from .models import load_model
 from .spaces import Box
 from .vector import VectorEnv
 
-ADROIT_REF_POINT = (0.0, -0.2, 0.2)   # fixed world point of the spatial algebra: inside the hand's workspace
 FRAME_SKIP = 5
 BOARD_Z_RANGE = (0.1, 0.25)           # adroit_hammer.py:374-376
 
@@ -48,10 +47,6 @@ def make_hammer_task(model, reward_type, frame_skip=FRAME_SKIP):
     t.nobs = int(m.nq) - 6 + 6 + 13
     t.dt = float(m.opt[0] * frame_skip)
     return t
-
-
-class _AdroitBackend(CudaBackend):
-    REF = ADROIT_REF_POINT
 
 
 def make_relocate_task(model, reward_type, frame_skip=FRAME_SKIP):
@@ -128,7 +123,7 @@ class _AdroitVectorEnv(VectorEnv):
         super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 3), ("penv", 7)),
                          action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32),                  # adroit_hammer.py:229-232
                          observation_space=Box(-np.inf, np.inf, shape=(int(t.nobs),), dtype=np.float64),
-                         backend_factory=backend_factory or _AdroitBackend, num_envs=num_envs, device=device,
+                         backend_factory=backend_factory or CudaBackend, num_envs=num_envs, device=device,
                          max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
                          n_substeps=frame_skip, kwargs=kwargs)
         self.init_qpos = torch.as_tensor(np.array(m.qpos0), dtype=torch.float32, device=self.device)   # MujocoEnv: data.qpos at load

@@ -44,6 +44,17 @@ FETCH_TASKS = {
 }
 N_SUBSTEPS = 20
 REF_POINT = (1.0, 0.75, 0.4)  # fixed world point the device spatial algebra is expressed about
+# the same point of the other families, inside each robot's workspace
+HAND_REF_POINT = (1.0, 0.9, 0.2)
+ADROIT_REF_POINT = (0.0, -0.2, 0.2)
+KITCHEN_REF_POINT = (-0.2, 0.3, 1.8)
+
+
+def reference_point(task):
+    """The fixed world point of a task's spatial algebra, by task kind: Fetch (0) and maze (1) REF_POINT, Hand (2, 3) HAND_REF_POINT,
+    Adroit (4-7) ADROIT_REF_POINT, Kitchen (8) KITCHEN_REF_POINT."""
+    k = int(task.kind)
+    return HAND_REF_POINT if k in (2, 3) else ADROIT_REF_POINT if 4 <= k <= 7 else KITCHEN_REF_POINT if k == 8 else REF_POINT
 
 
 def make_task_struct(model, cfg, reward_type, n_substeps=N_SUBSTEPS):
@@ -93,7 +104,8 @@ class CudaBackend:
         self.L = _lib.lib()
         blob = model.to_blob()
         h = ctypes.c_void_p()
-        ref = np.asarray(getattr(self, "REF", REF_POINT), dtype=np.float32)
+        self.ref = reference_point(task)
+        ref = np.asarray(self.ref, dtype=np.float32)
         # eq_data: NULL (keep the blob's equality data) or exactly neq x 11 doubles (include/b200sim.h); the C side cannot see the
         # length, so an empty override must become NULL here -- a pointer to a zero-length array would be read out of bounds
         eq = np.ascontiguousarray(eq_data, dtype=np.float64)

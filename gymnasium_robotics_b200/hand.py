@@ -20,7 +20,7 @@ import torch
 
 from . import rotations
 from ._lib import FetchTaskC
-from .fetch import CudaBackend, N_SUBSTEPS
+from .fetch import HAND_REF_POINT, CudaBackend, N_SUBSTEPS  # noqa: F401  (HAND_REF_POINT: re-exported)
 from .models import load_model
 from .spaces import Box, Dict as DictSpace
 from .vector import VectorEnv
@@ -46,7 +46,6 @@ HAND_TASKS = {
                               randomize_initial_rotation=False, ignore_z_target_rotation=True, distance_threshold=0.05),
 }
 TARGET_POSITION_RANGE = np.array([(-0.04, 0.04), (-0.06, 0.02), (0.0, 0.06)])
-HAND_REF_POINT = (1.0, 0.9, 0.2)   # fixed world point of the spatial algebra: inside the hand's workspace
 GOAL_USE_POS, GOAL_USE_ROT, GOAL_IGNORE_Z = 1, 2, 4
 
 
@@ -71,10 +70,6 @@ def make_hand_task(model, target_position, target_rotation, reward_type, distanc
     t.distance_threshold, t.rotation_threshold = float(distance_threshold), float(rotation_threshold)
     t.dt = float(m.opt[0] * n_substeps)
     return t
-
-
-class _HandBackend(CudaBackend):
-    REF = HAND_REF_POINT
 
 
 def _goal_space(ngoal, nobs):
@@ -121,7 +116,7 @@ class HandVectorEnv(VectorEnv):
         # "device": start pose and goal are drawn inside the library (b200sim_reset_hand_pose / _goal, csrc/reset_sample.cuh)
         super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 7)),
                          action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32), observation_space=_goal_space(7, t.nobs),
-                         backend_factory=backend_factory or _HandBackend, num_envs=num_envs, device=device,
+                         backend_factory=backend_factory or CudaBackend, num_envs=num_envs, device=device,
                          max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
                          n_substeps=n_substeps, kwargs=kwargs)
         lay = self.backend.layout
@@ -364,7 +359,7 @@ class HandReachVectorEnv(VectorEnv):
             t.tip_site[k] = m.site_id(name)
         super().__init__(model=m, task=t, fields=(("qpos", m.nq), ("qvel", m.nv), ("warm", m.nv), ("ctrl", m.nu), ("goal", 15)),
                          action_space=Box(-1.0, 1.0, shape=(int(m.nu),), dtype=np.float32), observation_space=_goal_space(15, t.nobs),
-                         backend_factory=backend_factory or _HandBackend, num_envs=num_envs, device=device,
+                         backend_factory=backend_factory or CudaBackend, num_envs=num_envs, device=device,
                          max_episode_steps=max_episode_steps, autoreset_mode=autoreset_mode, rng_mode=rng_mode,
                          n_substeps=n_substeps, kwargs=kwargs)
         # _env_setup (reach.py:286-296): initial joint angles, mj_forward, initial fingertip positions and palm position

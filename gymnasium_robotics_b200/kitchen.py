@@ -20,12 +20,11 @@ import numpy as np
 import torch
 
 from ._lib import FetchTaskC
-from .fetch import CudaBackend
+from .fetch import KITCHEN_REF_POINT, CudaBackend  # noqa: F401  (KITCHEN_REF_POINT: re-exported)
 from .models import load_franka_config, load_model
 from .spaces import Box
 from .vector import VectorEnv
 
-KITCHEN_REF_POINT = (-0.2, 0.3, 1.8)   # fixed world point of the spatial algebra: inside the robot's workspace
 FRAME_SKIP = 40
 # kitchen_env.py:27-45
 OBS_ELEMENT_INDICES = {
@@ -53,10 +52,6 @@ def make_kitchen_task(model, frame_skip=FRAME_SKIP):
     t.dt = float(model.opt[0] * frame_skip)
     t.penv_body = -1
     return t
-
-
-class _KitchenBackend(CudaBackend):
-    REF = KITCHEN_REF_POINT
 
 
 class KitchenVectorEnv(VectorEnv):
@@ -101,7 +96,7 @@ class KitchenVectorEnv(VectorEnv):
         if mesh_collision == "hull" and broadphase != "groups":
             raise ValueError("mesh_collision='hull' exists for the two-level broad phase only")
         self.broadphase = broadphase
-        factory = backend_factory or _KitchenBackend
+        factory = backend_factory or CudaBackend
 
         def make_backend(*args):
             prev = os.environ.get("B200SIM_KITCHEN_GROUPS")
@@ -122,7 +117,7 @@ class KitchenVectorEnv(VectorEnv):
                          backend_factory=make_backend, num_envs=num_envs, device=device, max_episode_steps=max_episode_steps,
                          autoreset_mode=autoreset_mode, rng_mode=rng_mode, n_substeps=frame_skip, kwargs=kwargs)
         self._can_terminate = bool(terminate_on_tasks_completed)
-        if self.rng_mode == "device" and not hasattr(self.backend, "set_obs_noise"):
+        if self.rng_mode == "device" and getattr(self.backend, "set_obs_noise", None) is None:
             self.backend.close()
             raise NotImplementedError("rng_mode='device' needs a backend that draws the observation noise in the step "
                                       f"(set_obs_noise, b200sim_set_obs_noise); {type(self.backend).__name__} has none")

@@ -317,7 +317,7 @@ class MazeVectorEnv(VectorEnv):
         # (_new_ant_rows) and the reset positions Ant-v5 measures distance_from_origin from
         self._ant_rows = self._ant_origin = None
         if self.ant is not None and t.touch_mode >= 2:
-            if not hasattr(self.backend, "set_ant_info"):
+            if getattr(self.backend, "set_ant_info", None) is None:
                 raise NotImplementedError(f"{type(self.backend).__name__} cannot run the Ant's keywords (no set_ant_info)")
             self._ant_params = self.ant.params()
             self._ant_origin = torch.zeros((self.num_envs, 2), dtype=torch.float32, device=self.device)
@@ -335,9 +335,9 @@ class MazeVectorEnv(VectorEnv):
         # step launch does it (b200sim_set_goal_redraw), rewriting the reward too
         self._goal_redraw_on = v3 and continuing_task and len(self.cells.goal_locations) > 1
         self._goal_update_seed = None
-        if self.rng_mode == "device" and self._goal_update_on and not hasattr(self.backend, "set_goal_update"):
+        if self.rng_mode == "device" and self._goal_update_on and getattr(self.backend, "set_goal_update", None) is None:
             raise NotImplementedError(f"{type(self.backend).__name__} cannot update goals on the device (no set_goal_update)")
-        if self.rng_mode == "device" and self._goal_redraw_on and not hasattr(self.backend, "set_goal_redraw"):
+        if self.rng_mode == "device" and self._goal_redraw_on and getattr(self.backend, "set_goal_redraw", None) is None:
             raise NotImplementedError(f"{type(self.backend).__name__} cannot redraw goals on the device (no set_goal_redraw)")
 
     # ------------------------------------------------------------------ sampling (MazeEnv.reset, maze_v4.py:299-358)

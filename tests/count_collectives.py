@@ -1,19 +1,18 @@
 """Dynamic proxy without a GPU: warp collectives (shuffles, ballots, __syncwarp) executed per kitchen sub-step by the flat-scan build and by
 the two-level broad-phase build, counted by the 32-lane fiber emulation (tests/hostsim/hostwarp.h scheduler rounds).
     PYTHONPATH=. python tests/count_collectives.py"""
-import numpy as np, torch, ctypes
-from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT, KitchenVectorEnv
+import functools
+import numpy as np, torch
+from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
 from gymnasium_robotics_b200.models import load_model
 from tests.hostsim_backend import HostSimBackend
 from tests import hostsim
 m = load_model("franka_kitchen")
 res={}
 for fl in ("warp_kitchen", "warp_kitchen_groups"):
-    class B(HostSimBackend):
-        REF = KITCHEN_REF_POINT; FLAVOR = fl
-    env = KitchenVectorEnv(num_envs=1, backend_factory=B, device="cpu", rng_mode="numpy", model=m)
+    env = KitchenVectorEnv(num_envs=1, backend_factory=functools.partial(HostSimBackend, flavor=fl), device="cpu", rng_mode="numpy", model=m)
     env.reset(seed=4)
-    L = hostsim.lib(fl); L.hostsim_collectives.restype = ctypes.c_long
+    L = hostsim.lib(fl)
     rng = np.random.default_rng(0)
     c0 = L.hostsim_collectives()
     for k in range(3):

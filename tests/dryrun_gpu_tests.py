@@ -11,27 +11,13 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHIM = '''
 import gymnasium_robotics_b200 as _p
-from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
-from gymnasium_robotics_b200.fetch import REF_POINT
-from gymnasium_robotics_b200.hand import HAND_REF_POINT
-from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT
 from tests.hostsim_backend import HostSimBackend
 
 
 def make_vec(env_id, num_envs=1, **kw):
-    ref, flavor = REF_POINT, None
-    if env_id.startswith("Adroit"):
-        ref = ADROIT_REF_POINT
-    elif env_id.startswith("Hand"):
-        ref = HAND_REF_POINT
-    elif env_id.startswith("Franka"):
-        ref, flavor = KITCHEN_REF_POINT, ("kitchen_hull" if kw.get("mesh_collision") == "hull" else "kitchen")
+    if env_id.startswith("Franka"):
         kw.setdefault("device", "cpu")
-
-    class B(HostSimBackend):
-        REF, FLAVOR = ref, flavor
-
-    kw.setdefault("backend_factory", B)
+    kw.setdefault("backend_factory", HostSimBackend)
     return _p.make_vec(env_id, num_envs=num_envs, **kw)
 '''
 
@@ -50,8 +36,7 @@ if __name__ == "__main__":
             for a, b in (('device="cuda"', 'device="cpu"'), (".cuda()", ".cpu()"), ('"cuda:0"', '"cpu"'), ("pytestmark = pytest.mark.gpu", "pytestmark = []"),
                          (".is_cuda", ".is_cpu"), ("import gymnasium_robotics_b200 as pkg", "import gpu_dryrun_shim as pkg"),
                          ("from gymnasium_robotics_b200 import make_vec", "from gpu_dryrun_shim import make_vec"),
-                         ("from gymnasium_robotics_b200.kitchen import _KitchenBackend, make_kitchen_task",
-                          "from gymnasium_robotics_b200.kitchen import make_kitchen_task\n    from tests.test_kitchen_host import KitchenHostBackend as _KitchenBackend"),
+                         ("from gymnasium_robotics_b200.fetch import CudaBackend", "from tests.hostsim_backend import HostSimBackend as CudaBackend"),
                          ("ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))", f'ROOT = "{ROOT}"')):
                 s = s.replace(a, b)
             names.append(os.path.join(tmp, os.path.basename(path)))

@@ -7,100 +7,154 @@ import subprocess
 
 import numpy as np
 
+from gymnasium_robotics_b200 import _lib
+from gymnasium_robotics_b200.mjcf import EQ_JOINT, GEOM_MESH
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(os.path.dirname(_HERE))
 _LIB = {}
 
 
 class FetchTaskC(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_int) for n in ("has_object", "block_gripper", "n_substeps", "reward_dense", "grip_site",
-                                             "obj_site", "frame_site", "nrobot")] + \
-               [("robot_qadr", ctypes.c_int * 16), ("robot_dadr", ctypes.c_int * 16), ("finger_qadr", ctypes.c_int * 2),
-                ("nobs", ctypes.c_int), ("distance_threshold", ctypes.c_float), ("dt", ctypes.c_float),
-                ("kind", ctypes.c_int), ("nact", ctypes.c_int), ("ngoal", ctypes.c_int), ("success_radius", ctypes.c_float),
-                ("obs_qpos_start", ctypes.c_int), ("vel_clip", ctypes.c_float),
-                ("obj_qadr", ctypes.c_int), ("obj_dadr", ctypes.c_int), ("goal_flags", ctypes.c_int),
-                ("rotation_threshold", ctypes.c_float), ("touch_mode", ctypes.c_int), ("tip_site", ctypes.c_int * 5),
-                ("penv_body", ctypes.c_int)] + \
-               [(n, ctypes.c_int) for n in ("st_qpos", "st_qvel", "st_warm", "st_ctrl", "st_mocap", "st_pose", "st_goal",
-                                             "st_stride", "st_penv")]
+    """FetchTask (csrc/fetch_task.cuh): b200sim_fetch_task_t and the state-record offsets b200sim_create adds to it."""
+    _fields_ = _lib.FetchTaskC._fields_ + [(n, ctypes.c_int) for n in ("st_qpos", "st_qvel", "st_warm", "st_ctrl", "st_mocap", "st_pose",
+                                                                       "st_goal", "st_stride", "st_penv")]
+
+
+class ObsNoiseKey(ctypes.Structure):
+    """ObsNoiseKey (csrc/fetch_task.cuh): one env's observation-noise stream in one launch."""
+    _fields_ = [("scale", ctypes.c_void_p), ("seed", ctypes.c_ulonglong), ("env", ctypes.c_uint), ("episode", ctypes.c_uint), ("t", ctypes.c_uint)]
+
+
+class AntInfoArgsC(ctypes.Structure):
+    """AntInfoArgs (csrc/fetch_task.cuh)"""
+    _fields_ = [(n, ctypes.c_float) for n in ("cf_lo", "cf_hi", "forward_w", "ctrl_w", "contact_w", "healthy_reward", "z_lo", "z_hi")] + \
+               [(n, ctypes.c_int) for n in ("v4", "survive_always", "contact_in_ctrl")] + [("rows", ctypes.c_void_p), ("origin", ctypes.c_void_p)]
+
+
+_WARP = ["-DB200_HOST_WARP", "-Wno-unknown-pragmas"]   # WARP_W == 32 on lock-step fibers (hostwarp.h): the lane-parallel code paths
+_KITCHEN, _GROUPS = ["-DB200_KITCHEN"], ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS"]
+# one row per emulated kernel build: flavor -> (library, g++ defines)
+#   False: the plain build; True: the 64-bit dof-mask build (models with more than 32 dofs, csrc/b200sim_wide.cu);
+#   "kitchen": the Franka-Kitchen kernel features with the flat-scan broad phase (csrc/b200sim_kitchen.cu); "kitchen_groups": the
+#   two-level broad phase (regrouped pair list, group table, csrc/b200sim_kitchen_groups.cu); "kitchen_flat": the groups build's data
+#   layout scanned in one level, the bit-exact A/B reference of the two-level scan; "kitchen_hull": the groups build plus the
+#   support-map narrow phase for mesh geoms (csrc/b200sim_kitchen_hull.cu); "ant": the Ant's keywords and info (csrc/b200sim_ant.cu);
+#   "warp*": those builds on the 32-lane emulated warp; "warp_timing" with the stage timer's collective counts
+FLAGS = {False: ("libhostsim.so", []), True: ("libhostsim_wide.so", ["-DB200_WIDE"]),
+         "kitchen": ("libhostsim_kitchen.so", _KITCHEN), "kitchen_groups": ("libhostsim_kitchen_groups.so", _GROUPS),
+         "kitchen_flat": ("libhostsim_kitchen_flat.so", _GROUPS + ["-DB200_KITCHEN_FLATSCAN"]),
+         "kitchen_hull": ("libhostsim_kitchen_hull.so", _GROUPS + ["-DB200_HULL"]), "ant": ("libhostsim_ant.so", ["-DB200_ANT"]),
+         "warp": ("libhostsim_warp.so", _WARP), "warp_wide": ("libhostsim_warp_wide.so", _WARP + ["-DB200_WIDE"]),
+         "warp_kitchen": ("libhostsim_warp_kitchen.so", _WARP + _KITCHEN), "warp_kitchen_groups": ("libhostsim_warp_kitchen_groups.so", _WARP + _GROUPS),
+         "warp_kitchen_hull": ("libhostsim_warp_kitchen_hull.so", _WARP + _GROUPS + ["-DB200_HULL"]),
+         "warp_timing": ("libhostsim_warp_timing.so", _WARP + ["-DB200_STAGE_TIMING"])}
+FLAVORS = tuple(f for f in FLAGS if f != "warp_timing")   # what the package build compiles; tests/count_stage_collectives.py builds the last
+_SRCS = [os.path.join(_HERE, "hostsim.cpp"), os.path.join(_HERE, "hostwarp.h")] + \
+        [os.path.join(_ROOT, "gymnasium_robotics_b200", "csrc", f) for f in ("sim_core.cuh", "dmodel.h", "fetch_task.cuh", "reset_sample.cuh")] + \
+        [os.path.join(_ROOT, "include", f) for f in ("b200sim_model.h", "b200sim.h")]
+
+
+def host_flavor(model, task):
+    """The flavor that emulates the kernel build b200sim_create picks for (model, task) (csrc/b200sim.cu): a mesh geom -> the hull build;
+    a joint equality or a condim-6 pair -> a kitchen build (flat scan when B200SIM_KITCHEN_GROUPS=0, else the two-level broad phase);
+    more than 32 dofs -> the wide build; a maze task with touch_mode 2..4 -> the ant build; else the plain build."""
+    if (np.asarray(model.geom_type) == GEOM_MESH).any():
+        return "kitchen_hull"
+    if (np.asarray(model.eq_type)[:model.neq] == EQ_JOINT).any() or (np.asarray(model.pair_condim) == 6).any():
+        return "kitchen" if os.environ.get("B200SIM_KITCHEN_GROUPS") == "0" else "kitchen_groups"
+    if model.nv > 32:
+        return True
+    return "ant" if task.kind == 1 and task.touch_mode >= 2 else False
 
 
 def build(force=False, wide=False):
-    """wide = True: the 64-bit dof-mask build (models with more than 32 dofs, -DB200_WIDE as in csrc/b200sim_wide.cu);
-    wide = "kitchen": the bring-up build of the Franka-Kitchen kernel features (-DB200_KITCHEN, DESIGN.md section 7);
-    wide = "kitchen_groups": that build with the two-level broad phase (-DB200_KITCHEN_GROUPS: regrouped pair list, group table);
-    wide = "kitchen_flat": the groups build's data layout scanned in one level, the bit-exact A/B reference of the two-level scan
-    (-DB200_KITCHEN_FLATSCAN)"""
-    out = os.path.join(_HERE, {True: "libhostsim_wide.so", "kitchen": "libhostsim_kitchen.so", "kitchen_groups": "libhostsim_kitchen_groups.so",
-                               "kitchen_flat": "libhostsim_kitchen_flat.so", "warp": "libhostsim_warp.so", "warp_wide": "libhostsim_warp_wide.so",
-                               "warp_kitchen_groups": "libhostsim_warp_kitchen_groups.so", "warp_kitchen": "libhostsim_warp_kitchen.so", "warp_timing": "libhostsim_warp_timing.so",
-                               "kitchen_hull": "libhostsim_kitchen_hull.so", "warp_kitchen_hull": "libhostsim_warp_kitchen_hull.so"}.get(wide, "libhostsim.so"))
-    srcs = [os.path.join(_HERE, "hostsim.cpp")] + [os.path.join(_ROOT, "gymnasium_robotics_b200", "csrc", f)
-                                                   for f in ("sim_core.cuh", "dmodel.h", "fetch_task.cuh")] + \
-           [os.path.join(_ROOT, "include", "b200sim_model.h"), os.path.join(_ROOT, "include", "b200sim.h"), os.path.join(_HERE, "hostwarp.h"),
-            os.path.join(_ROOT, "gymnasium_robotics_b200", "csrc", "reset_sample.cuh")]
+    """Compile the library of flavor `wide` (a key of FLAGS) when it is older than a source.  Several processes may get here at once
+    (the 2-rank gloo tests, pytest-xdist): one compiles under a file lock into a temporary name and renames it into place, the others
+    wait and then find the library fresh."""
+    name, defines = FLAGS[wide]
+    out = os.path.join(_HERE, name)
+
     def stale():
-        return force or not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(s) for s in srcs)
+        return force or not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(s) for s in _SRCS)
 
     if stale():
-        # several processes may get here at once (the 2-rank gloo tests, pytest-xdist): one compiles under a file lock into a
-        # temporary name and renames it into place, the others wait and then find the library fresh
         import fcntl
 
         with open(out + ".lock", "w") as lk:
             fcntl.flock(lk, fcntl.LOCK_EX)
             if stale():
                 tmp = f"{out}.{os.getpid()}.tmp"
-                subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unused-function"] +
-                                      ({"kitchen": ["-DB200_KITCHEN"], "kitchen_groups": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS"],
-                                        "kitchen_flat": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS", "-DB200_KITCHEN_FLATSCAN"],
-                                        # WARP_W == 32 on lock-step fibers (hostwarp.h): the lane-parallel code paths themselves
-                                        "warp": ["-DB200_HOST_WARP", "-Wno-unknown-pragmas"],
-                                        "warp_wide": ["-DB200_HOST_WARP", "-DB200_WIDE", "-Wno-unknown-pragmas"],
-                                        "warp_timing": ["-DB200_HOST_WARP", "-DB200_STAGE_TIMING", "-Wno-unknown-pragmas"],
-                                        "warp_kitchen": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-Wno-unknown-pragmas"],
-                                        "warp_kitchen_groups": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
-                                                                "-Wno-unknown-pragmas"],
-                                        # the kitchen groups build + the support-map narrow phase for mesh geoms (csrc/b200sim_kitchen_hull.cu)
-                                        "kitchen_hull": ["-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS", "-DB200_HULL"],
-                                        "warp_kitchen_hull": ["-DB200_HOST_WARP", "-DB200_KITCHEN", "-DB200_KITCHEN_GROUPS",
-                                                              "-DB200_HULL", "-Wno-unknown-pragmas"]}.get(wide) or
-                                       (["-DB200_WIDE"] if wide else [])) + ["-o", tmp, srcs[0]])
+                subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unused-function"] + defines + ["-o", tmp, _SRCS[0]])
                 os.replace(tmp, out)
                 force = False
     return out
 
 
 def lib(wide=False):
+    """The library of flavor `wide`, every hostsim_* function it exports with its argument and result types."""
     if _LIB.get(wide) is None:
         L = ctypes.CDLL(build(wide=wide))
-        L.hostsim_create.restype = ctypes.c_void_p
-        L.hostsim_create.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
-        L.hostsim_scratch.restype = ctypes.POINTER(ctypes.c_float)
-        L.hostsim_scratch.argtypes = [ctypes.c_void_p]
-        for f in ("hostsim_destroy", "hostsim_forward", "hostsim_kinematics"):
-            getattr(L, f).argtypes = [ctypes.c_void_p]
-            getattr(L, f).restype = None
-        L.hostsim_step.argtypes = [ctypes.c_void_p, ctypes.c_int]
-        L.hostsim_step.restype = None
-        L.hostsim_offset.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
-        L.hostsim_scr_words.argtypes = [ctypes.c_void_p]
-        L.hostsim_env_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 7
-        L.hostsim_spd.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
-        L.hostsim_spd.restype = ctypes.c_int
-        for f in ("hostsim_collide", "hostsim_problem", "hostsim_jv", "hostsim_build_h"):
-            getattr(L, f).argtypes = [ctypes.c_void_p, ctypes.c_int]
-            getattr(L, f).restype = None
-        L.hostsim_model_offset.argtypes = [ctypes.c_void_p, ctypes.c_char_p]
-        L.hostsim_model.restype = ctypes.POINTER(ctypes.c_uint32)
-        L.hostsim_model.argtypes = [ctypes.c_void_p]
-        L.hostsim_model_words.argtypes = [ctypes.c_void_p]
-        L.hostsim_layout.argtypes = [ctypes.c_void_p]
-        L.hostsim_layout.restype = None
+        vp, ci, cu, cf, cu64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint, ctypes.c_float, ctypes.c_ulonglong
+        defines = FLAGS[wide][1]
+        step_extra = [vp] if "-DB200_KITCHEN" in defines or "-DB200_ANT" in defines else []   # the noise key / the Ant's arguments
+        sigs = {"hostsim_create": (vp, [ctypes.c_char_p, ctypes.c_size_t, vp, vp, ci, ci]),
+                "hostsim_destroy": (None, [vp]), "hostsim_scratch": (ctypes.POINTER(ctypes.c_float), [vp]),
+                "hostsim_scr_words": (ci, [vp]), "hostsim_npair": (ci, [vp]), "hostsim_nbgrp": (ci, [vp]),
+                "hostsim_offset": (ci, [vp, ctypes.c_char_p]), "hostsim_model_offset": (ci, [vp, ctypes.c_char_p]),
+                "hostsim_forward": (None, [vp]), "hostsim_kinematics": (None, [vp]), "hostsim_step": (None, [vp, ci]),
+                "hostsim_collide": (None, [vp, ci]), "hostsim_problem": (None, [vp, ci]), "hostsim_jv": (None, [vp, ci]),
+                "hostsim_build_h": (None, [vp, ci]),
+                "hostsim_model": (ctypes.POINTER(ctypes.c_uint32), [vp]), "hostsim_model_words": (ci, [vp]), "hostsim_hot_words": (ci, [vp]),
+                "hostsim_layout": (None, [vp]), "hostsim_task_size": (ci, []),
+                "hostsim_env_step": (ci, [vp, vp, ci, ci] + [vp] * 7 + step_extra),
+                "hostsim_spd": (ci, [ci, ci, vp, vp, cf, vp, vp]),
+                "hostsim_philox4x32_10": (None, [vp] * 3),
+                "hostsim_fetch_reset_record": (None, [vp, cu64, cu, cu, vp, ci, ci, ci, vp]),
+                "hostsim_uniform_reset_record": (None, [vp, cu64, cu, cu, vp, ci, vp]),
+                "hostsim_maze_reset_record": (None, [vp, vp, vp, cu64, cu, cu, vp, ci, ci, ci, vp]),
+                "hostsim_hand_pose_record": (None, [vp, vp, cu64, cu, cu, cu, vp, ci, ci, ci, ci, vp]),
+                "hostsim_hand_goal": (None, [vp, vp, cu64, cu, cu, ci, ci, vp]),
+                "hostsim_reach_reset_record": (None, [vp, cu64, cu, cu, vp, ci, ci, vp]),
+                "hostsim_check_record": (ci, [vp, ci, vp, vp]),
+                "hostsim_maze_goal_update": (ci, [vp, ci, cf, cf, cf, cu64, cu, cu, cu, vp, vp]),
+                "hostsim_maze_goal_redraw": (ci, [vp, ci, cf, cf, cf, ci, cu64, cu, cu, cu, vp, vp, vp]),
+                "hostsim_kitchen_noise": (None, [cu64, cu, cu, cu, vp]),       # kitchen flavors
+                "hostsim_collectives": (ctypes.c_long, []),                    # warp flavors
+                "hostsim_stage_rounds": (ci, [ctypes.POINTER(ctypes.c_longlong), ci])}   # warp_timing
+        for name, (res, args) in sigs.items():
+            f = getattr(L, name, None)      # (a function of some flavors only is absent from the others)
+            if f is not None:
+                f.restype, f.argtypes = res, args
         assert L.hostsim_task_size() == ctypes.sizeof(FetchTaskC)
         _LIB[wide] = L
     return _LIB[wide]
+
+
+def goal_update(goal_xy, scaling, noise, radius, seed, env, episode, step, ach, goal):
+    """rs_maze_goal_update on the host: (new goal as float32 [2], candidates drawn)."""
+    g = np.ascontiguousarray(goal_xy, dtype=np.float32)
+    a, out = np.asarray(ach, dtype=np.float32).copy(), np.asarray(goal, dtype=np.float32).copy()
+    n = lib().hostsim_maze_goal_update(g.ctypes.data, len(g), float(scaling), float(noise), float(radius), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                       int(env), int(episode), int(step), a.ctypes.data, out.ctypes.data)
+    return out, n
+
+
+def goal_redraw(goal_xy, scaling, noise, radius, dense, seed, env, episode, step, ach, goal):
+    """rs_maze_goal_redraw on the host: (new goal as float32 [2], reward against it as float32 or None when the goal stays)."""
+    g = np.ascontiguousarray(goal_xy, dtype=np.float32)
+    a, out, r = np.asarray(ach, dtype=np.float32).copy(), np.asarray(goal, dtype=np.float32).copy(), np.zeros(1, dtype=np.float32)
+    changed = lib().hostsim_maze_goal_redraw(g.ctypes.data, len(g), float(scaling), float(noise), float(radius), int(bool(dense)),
+                                             int(seed) & 0xFFFFFFFFFFFFFFFF, int(env), int(episode), int(step), a.ctypes.data, out.ctypes.data,
+                                             r.ctypes.data)
+    return out, (r[0] if changed else None)
+
+
+def kitchen_noise(seed, env, episode, t):
+    """The 59 uniforms in [-1, 1) of the kitchen observation-noise stream (seed; env, episode, step t), float32 [59]."""
+    out = np.zeros(59, dtype=np.float32)
+    lib("kitchen").hostsim_kitchen_noise(int(seed) & 0xFFFFFFFFFFFFFFFF, int(env), int(episode), int(t), out.ctypes.data)
+    return out
 
 
 def spd(flavor, nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
@@ -205,12 +259,13 @@ class HostSim:
     def step(self, n=1):
         self._L.hostsim_step(self._h, int(n))
 
-    def env_step(self, task, mode, nraw, st, action, nobs, ngoal=3):
+    def env_step(self, task, mode, nraw, st, action, nobs, ngoal=3, *extra):
+        """One env's launch; `extra`: the kitchen flavors' noise key or the ant flavor's arguments (hostsim_env_step)."""
         obs = np.zeros(nobs, dtype=np.float32)
         ag, dg = np.zeros(ngoal, dtype=np.float32), np.zeros(ngoal, dtype=np.float32)
         rew, suc = np.zeros(1, dtype=np.float32), np.zeros(1, dtype=np.float32)
         a = np.zeros(max(32, len(action)), dtype=np.float32)
         a[:len(action)] = action
         it = self._L.hostsim_env_step(self._h, ctypes.byref(task), mode, nraw, st.ctypes.data, a.ctypes.data, obs.ctypes.data,
-                                      ag.ctypes.data, dg.ctypes.data, rew.ctypes.data, suc.ctypes.data)
+                                      ag.ctypes.data, dg.ctypes.data, rew.ctypes.data, suc.ctypes.data, *extra)
         return obs, ag, dg, float(rew[0]), float(suc[0]), it

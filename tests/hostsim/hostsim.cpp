@@ -139,11 +139,31 @@ const uint32_t* hostsim_model(void* p) { return ((HostSim*)p)->model.data(); }
 // this flavor's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE
 void hostsim_layout(int* out) { out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE; }
 int hostsim_task_size() { return (int)sizeof(FetchTask); }
+// one env's launch.  The kitchen flavors take `noise`, the env's observation-noise key as the step kernel builds it (NULL:
+// noise-free); the ant flavor takes `a`, the Ant's keywords as b200sim_set_ant_info leaves them with rows / origin pointing at this
+// env's info row [9] / reset position [2] (or NULL), and runs what fetch_kernel_ant's lane 0 runs after the step (ant_info).  Like
+// fetch_env_step's, these parameters exist in those flavors only.
 int hostsim_env_step(void* p, const FetchTask* t, int mode, int nraw, float* st, const float* action, float* obs, float* achieved,
-                     float* desired, float* reward, float* success) {
+                     float* desired, float* reward, float* success
+#ifdef B200_KITCHEN
+                     , const ObsNoiseKey* noise
+#endif
+#ifdef B200_ANT
+                     , const AntInfoArgs* a
+#endif
+                     ) {
   int it = 0;
   warp_call(((HostSim*)p)->ctx, [&](const Ctx& c) {
+#if defined(B200_KITCHEN)
+    fetch_env_step<HOST_NVP>(c, *t, true, mode, nraw, st, action, obs, achieved, desired, reward, success, &it, noise);
+#elif defined(B200_ANT)
+    AntForces f = {a->cf_lo, a->cf_hi, 0.f};
+    fetch_env_step<HOST_NVP>(c, *t, true, mode, nraw, st, action, obs, achieved, desired, reward, success, &it, &f);
+    if (c.lane == 0)
+      ant_info(c, *t, *a, mode, mode == MODE_STEP ? t->n_substeps > 0 : (mode == MODE_RAW && nraw > 0), st, action, f.sq, 0);
+#else
     fetch_env_step<HOST_NVP>(c, *t, true, mode, nraw, st, action, obs, achieved, desired, reward, success, &it);
+#endif
   });
   return it;
 }
@@ -208,6 +228,29 @@ extern "C" void hostsim_reach_reset_record(const b200sim_reach_reset_t* p, unsig
                                            int stride, int st_goal, float* rec) {
   rs_reach_reset_record(*p, seed, env, episode, rest, stride, st_goal, rec);
 }
+// the maze goal update of b200sim_set_goal_update: goal [2] in/out; returns the number of candidates drawn (0: the goal stays)
+extern "C" int hostsim_maze_goal_update(const float* goal_xy, int n_goal, float scaling, float noise, float radius, unsigned long long seed,
+                                        unsigned env, unsigned episode, unsigned step, const float* ach, float* goal) {
+  return rs_maze_goal_update(goal_xy, n_goal, scaling, noise, radius, seed, env, episode, step, ach, goal);
+}
+// AntMaze-v3's goal redraw of b200sim_set_goal_redraw: goal [2] in/out, reward out (written only when the goal changed); returns 1
+// when the goal changed
+extern "C" int hostsim_maze_goal_redraw(const float* goal_xy, int n_goal, float scaling, float noise, float radius, int dense,
+                                        unsigned long long seed, unsigned env, unsigned episode, unsigned step, const float* ach, float* goal,
+                                        float* reward) {
+  return rs_maze_goal_redraw(goal_xy, n_goal, scaling, noise, radius, dense, seed, env, episode, step, ach, goal, reward);
+}
+#ifdef B200_KITCHEN
+// the 59 uniforms in [-1, 1) of the stream (seed; env, episode, step t), entry j = word j % 4 of block j / 4 (rs_obs_noise_block):
+// what the kitchen step kernel scales and adds
+extern "C" void hostsim_kitchen_noise(unsigned long long seed, unsigned env, unsigned episode, unsigned t, float* out) {
+  for (int b = 0; 4 * b < 59; b++) {
+    float u[4];
+    rs_obs_noise_block(seed, env, episode, t, (uint32_t)b, u);
+    for (int w = 0; w < 4 && 4 * b + w < 59; w++) out[4 * b + w] = u[w];
+  }
+}
+#endif
 extern "C" int hostsim_check_record(float* rec, int stride, const float* rest, const b200sim_keep_t* keep) {
   b200sim_keep_t k;
   k.n = 0;

@@ -3,6 +3,7 @@ collectives run in ascending, descending and shuffled order in three separate pr
 shared-memory race between lanes (the CPU stand-in for compute-sanitizer racecheck).  Prints one digest per family and order:
     PYTHONPATH=. python tests/lane_order_check.py            # runs the three orders and compares
 """
+import functools
 import hashlib
 import os
 import subprocess
@@ -21,11 +22,7 @@ def digests():
 
     out = {}
     for env_id, ref, flavor1, flavor32, warm, tol in CASES:
-        class W1(HostSimBackend):
-            REF, FLAVOR = ref, flavor1
-
-        class W32(HostSimBackend):
-            REF, FLAVOR = ref, flavor32
+        W1, W32 = (functools.partial(HostSimBackend, flavor=f) for f in (flavor1, flavor32))
 
         kw = dict(experimental=True) if env_id.startswith("Franka") else {}
         env = pkg.make_vec(env_id, num_envs=1, backend_factory=W1, rng_mode="numpy", **kw)

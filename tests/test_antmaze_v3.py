@@ -18,8 +18,8 @@ from gymnasium_robotics_b200._lib import MazeResetC
 from gymnasium_robotics_b200.maze import MAPS, NOISE, SUCCESS_RADIUS, MazeCells, MazeVectorEnv
 from tests import hostsim
 from tests.antmaze_v3_oracle import MazeResetLogicV3, OracleAntMazeV3Env
-from tests.hostsim.ant_info import AntInfoHostBackend
-from tests.hostsim.maze_redraw import GoalRedrawHostBackend, goal_redraw
+from tests.hostsim import goal_redraw
+from tests.hostsim_backend import HostSimBackend
 from tests.test_ant_info import V4_KEYS
 from tests.test_reset_device import M32, philox4x32_10, py_maze_draw, u01
 
@@ -29,13 +29,9 @@ V3_IDS = [f"AntMaze_{m}{s}-v3" for m in ("UMaze", "Open", "Open_Diverse_G", "Ope
 STEP_KEYS = V4_KEYS | {"_" + k for k in V4_KEYS} | {"solver_info"}
 
 
-class V3HostBackend(GoalRedrawHostBackend, AntInfoHostBackend):
-    """The host emulation of a v3 handle: the ant kernel build (Ant-v4 info) with b200sim_set_goal_redraw."""
-
-
 def mk(env_id="AntMaze_Large-v3", n=3, **kw):
     kw.setdefault("rng_mode", "numpy")
-    return pkg.make_vec(env_id, num_envs=n, backend_factory=V3HostBackend, **kw)
+    return pkg.make_vec(env_id, num_envs=n, backend_factory=HostSimBackend, **kw)
 
 
 def _goals(env):
@@ -84,7 +80,7 @@ def test_registry_and_every_id_builds():
     env.reset(seed=0)
     assert set(env.step(_zeros(env))[4]) == {"solver_info"}
     env.close()
-    assert not pkg.make_vec("AntMaze_UMaze-v4", num_envs=1, backend_factory=AntInfoHostBackend).ant_info
+    assert not pkg.make_vec("AntMaze_UMaze-v4", num_envs=1, backend_factory=HostSimBackend).ant_info
 
 
 @pytest.mark.parametrize("kw,exc", [(dict(reset_target=True), TypeError), (dict(reset_target=False), TypeError),
@@ -98,11 +94,11 @@ def test_refused_keywords(kw, exc):
 
 def test_v3_is_the_ant_agents_and_v4_stays_the_default():
     with pytest.raises(ValueError):
-        MazeVectorEnv("UMaze", agent="point", maze_version=3, backend_factory=V3HostBackend)
+        MazeVectorEnv("UMaze", agent="point", maze_version=3, backend_factory=HostSimBackend)
     with pytest.raises(ValueError):
-        MazeVectorEnv("UMaze", maze_version=5, backend_factory=V3HostBackend)
+        MazeVectorEnv("UMaze", maze_version=5, backend_factory=HostSimBackend)
     with pytest.raises(ValueError):
-        MazeVectorEnv("UMaze", maze_version=3, ant_version=5, backend_factory=V3HostBackend)
+        MazeVectorEnv("UMaze", maze_version=3, ant_version=5, backend_factory=HostSimBackend)
     env = mk("AntMaze_UMaze-v4", n=1)
     assert env.maze_version == 4 and env.separation == 2.0 and not env.ant_info
     env.close()
@@ -156,9 +152,6 @@ def test_numpy_resets_match_the_restatement_and_can_start_in_the_goal_cell():
 
 def _c_maze_draw(goal_xy, reset_xy, scaling, separation, seed, env, episode):
     L = hostsim.lib()
-    L.hostsim_maze_reset_record.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_ulonglong, ctypes.c_uint, ctypes.c_uint,
-                                            ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    L.hostsim_maze_reset_record.restype = None
     p = MazeResetC()
     p.n_goal, p.n_reset, p.scaling, p.noise, p.separation = len(goal_xy), len(reset_xy), scaling, NOISE, separation
     g, r = np.ascontiguousarray(goal_xy, dtype=f32), np.ascontiguousarray(reset_xy, dtype=f32)

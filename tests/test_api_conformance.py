@@ -10,37 +10,15 @@ import pytest
 import torch
 
 import gymnasium_robotics_b200 as pkg
-from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
-from gymnasium_robotics_b200.fetch import REF_POINT
-from gymnasium_robotics_b200.hand import HAND_REF_POINT
-from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT
 from tests.hostsim_backend import HostSimBackend
 
 
-class FetchHostBackend(HostSimBackend):        # (module-level classes: the pickled constructor call names its backend factory)
-    REF, FLAVOR = REF_POINT, None
-
-
-class HandHostBackend(HostSimBackend):
-    REF, FLAVOR = HAND_REF_POINT, None
-
-
-class AdroitHostBackend(HostSimBackend):
-    REF, FLAVOR = ADROIT_REF_POINT, None
-
-
-class KitchenHostBackend(HostSimBackend):
-    REF, FLAVOR = KITCHEN_REF_POINT, "kitchen"
+class KitchenHostBackend(HostSimBackend):     # (module-level class: the pickled constructor call names its backend factory)
+    FLAVOR = "kitchen"
 
 
 def _factory(env_id):
-    if env_id.startswith("Adroit"):
-        return AdroitHostBackend
-    if env_id.startswith("Hand"):
-        return HandHostBackend
-    if env_id.startswith("Franka"):
-        return KitchenHostBackend
-    return FetchHostBackend
+    return KitchenHostBackend if env_id.startswith("Franka") else HostSimBackend
 
 
 # (id, goal-env?, action dim, observation dim)
@@ -60,7 +38,8 @@ def _make(env_id, n=2, **kw):
     kw.setdefault("rng_mode", "numpy")
     if env_id.startswith("Franka"):
         kw.setdefault("device", "cpu")
-    return pkg.make_vec(env_id, num_envs=n, backend_factory=_factory(env_id), **kw)
+    kw.setdefault("backend_factory", _factory(env_id))
+    return pkg.make_vec(env_id, num_envs=n, **kw)
 
 
 def _leaves(x, prefix=""):

@@ -65,15 +65,11 @@ def _run_mixed(rank, world, port, n_local, steps, out_q):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import gymnasium_robotics_b200 as pkg
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
     from gymnasium_robotics_b200.sharding import gather_mixed_outputs, mixed_batch_assignment
     from tests.hostsim_backend import HostSimBackend
 
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
     env_id = mixed_batch_assignment(["AdroitHandHammer-v2", "AdroitHandRelocate-v2"], world)[rank]
-    env = pkg.make_vec(env_id, num_envs=n_local, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec(env_id, num_envs=n_local, backend_factory=HostSimBackend, rng_mode="numpy")
     env.reset(seed=[7 + rank * n_local + i for i in range(n_local)])
     rng = np.random.default_rng(rank)
     for _ in range(steps):

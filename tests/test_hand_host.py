@@ -5,22 +5,20 @@ import pytest
 import torch
 
 import gymnasium_robotics_b200 as pkg
-from gymnasium_robotics_b200.hand import HandVectorEnv, HAND_REF_POINT
+from gymnasium_robotics_b200.hand import HandVectorEnv
 from gymnasium_robotics_b200.models import load_model
 from oracle.hand_env import OracleHandBlockEnv
 from tests.hostsim_backend import HostSimBackend
 
 
-class HandHostBackend(HostSimBackend):
-    REF = HAND_REF_POINT
 
 
 def make(task="HandManipulateBlockRotateXYZ", n=1, **kw):
-    return HandVectorEnv(task, num_envs=n, backend_factory=HandHostBackend, rng_mode="numpy", **kw)
+    return HandVectorEnv(task, num_envs=n, backend_factory=HostSimBackend, rng_mode="numpy", **kw)
 
 
 def test_spaces_and_ids():
-    env = pkg.make_vec("HandManipulateBlockRotateXYZ-v1", num_envs=2, backend_factory=HandHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("HandManipulateBlockRotateXYZ-v1", num_envs=2, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.single_action_space.shape == (20,)
     assert env.single_observation_space["observation"].shape == (61,)
     assert env.single_observation_space["achieved_goal"].shape == (7,)
@@ -104,9 +102,9 @@ def test_touch_sensor_observation_tracks_oracle():
     """HandManipulateBlockRotateXYZ_ContinuousTouchSensors-v1 / _BooleanTouchSensors-v1: 92 extra observation entries."""
     model = load_model("hand_block_touch")
     assert model.nsensor == 92
-    env = pkg.make_vec("HandManipulateBlockRotateXYZ_ContinuousTouchSensors-v1", num_envs=1, backend_factory=HandHostBackend,
+    env = pkg.make_vec("HandManipulateBlockRotateXYZ_ContinuousTouchSensors-v1", num_envs=1, backend_factory=HostSimBackend,
                        rng_mode="numpy")
-    envb = pkg.make_vec("HandManipulateBlockRotateXYZ_BooleanTouchSensors-v1", num_envs=1, backend_factory=HandHostBackend,
+    envb = pkg.make_vec("HandManipulateBlockRotateXYZ_BooleanTouchSensors-v1", num_envs=1, backend_factory=HostSimBackend,
                         rng_mode="numpy")
     assert env.single_observation_space["observation"].shape == (153,)
     orc = OracleHandBlockEnv(model=model, touch_get_obs="sensordata")
@@ -142,7 +140,7 @@ def test_hand_reach_matches_oracle():
     from oracle.hand_env import OracleHandReachEnv
 
     model = load_model("hand_reach")
-    env = pkg.make_vec("HandReach-v3", num_envs=2, backend_factory=HandHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("HandReach-v3", num_envs=2, backend_factory=HostSimBackend, rng_mode="numpy")
     assert isinstance(env, HandReachVectorEnv) and env.max_episode_steps == 50
     assert env.single_observation_space["observation"].shape == (63,) and env.single_action_space.shape == (20,)
     orc = OracleHandReachEnv(model=model)
@@ -170,7 +168,7 @@ def test_pen_env_matches_oracle():
     """HandManipulatePen*-v1: capsule object, no initial rotation randomisation, z rotation ignored in the goal distance,
     5 cm position threshold (manipulate_pen.py:216-235)."""
     model = load_model("hand_pen")
-    env = pkg.make_vec("HandManipulatePenRotate-v1", num_envs=1, backend_factory=HandHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("HandManipulatePenRotate-v1", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.ignore_z_target_rotation and env.distance_threshold == 0.05 and not env.randomize_initial_rotation
     orc = OracleHandBlockEnv(model=model, target_position="ignore", target_rotation="xyz", randomize_initial_rotation=False,
                              ignore_z_target_rotation=True, distance_threshold=0.05)
@@ -198,7 +196,7 @@ def test_pen_env_matches_oracle():
         np.testing.assert_allclose(obs["observation"][0, 54:57].double().numpy(), oobs["observation"][54:57], atol=2e-3)
         assert float(rew[0]) == float(orew)
     # ignore-z goal distance: dense reward on random pose pairs against the oracle's numpy restatement
-    envd = pkg.make_vec("HandManipulatePenRotateDense-v1", num_envs=1, backend_factory=HandHostBackend, rng_mode="numpy")
+    envd = pkg.make_vec("HandManipulatePenRotateDense-v1", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     orcd = OracleHandBlockEnv(model=model, target_position="ignore", target_rotation="xyz", reward_type="dense",
                               randomize_initial_rotation=False, ignore_z_target_rotation=True, distance_threshold=0.05)
     ag, dg = rng.normal(size=(32, 7)), rng.normal(size=(32, 7))
@@ -226,7 +224,7 @@ def test_egg_env_matches_oracle():
     """HandManipulateEgg*-v1 (manipulate_egg.py:214-235): ellipsoid object through the general convex collider, otherwise
     the block env's defaults."""
     model = load_model("hand_egg")
-    env = pkg.make_vec("HandManipulateEggRotate-v1", num_envs=1, backend_factory=HandHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("HandManipulateEggRotate-v1", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert not env.ignore_z_target_rotation and env.distance_threshold == 0.01 and env.randomize_initial_rotation
     orc = OracleHandBlockEnv(model=model, target_position="ignore", target_rotation="xyz")
     obs, _ = env.reset(seed=21)
@@ -263,15 +261,11 @@ def test_adroit_hammer_env_matches_oracle():
     """AdroitHandHammer-v2 on the wide build (33 dofs: 64-bit dof masks, bordered Cholesky; emulated here with -DB200_WIDE):
     reset (board height from the same PCG64 draw), env-steps from injected oracle states, dense and sparse reward,
     get/set_env_state round trip (adroit_hammer.py:291-402)."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
     from oracle.adroit_env import OracleAdroitHammerEnv
-
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
 
     m = load_model("adroit_hammer")
     assert m.nv == 33 and m.nu == 26
-    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.single_observation_space.shape == (46,) and env.single_action_space.shape == (26,) and env.max_episode_steps == 200
     orc = OracleAdroitHammerEnv(m, noslip=False)
     obs, info = env.reset(seed=4)
@@ -304,7 +298,7 @@ def test_adroit_hammer_env_matches_oracle():
         assert not bool(te.any()) and not bool(tr.any())
     assert np.median(errs) < 5e-6
     # sparse reward ids and the state round trip
-    envs = pkg.make_vec("AdroitHandHammerSparse-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    envs = pkg.make_vec("AdroitHandHammerSparse-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     envs.reset(seed=4)
     _, r, *_ = envs.step(np.zeros((1, 26), dtype=np.float32))
     assert float(r[0]) == pytest.approx(-0.1)
@@ -313,21 +307,17 @@ def test_adroit_hammer_env_matches_oracle():
     st2 = env.get_env_state()
     assert torch.equal(st["qpos"], st2["qpos"]) and torch.equal(st["board_pos"], st2["board_pos"]) and o1.shape == (1, 46)
     with pytest.raises(ValueError):
-        pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=AdroitHostBackend, reward_type="shaped")
+        pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=HostSimBackend, reward_type="shaped")
 
 
 def test_adroit_relocate_env_matches_oracle():
     """AdroitHandRelocate-v2 (36 dofs, wide build): five reset draws in the reference's order (ball x, y; target x, y, z),
     env-steps from injected oracle states, reward / success, state round trip (adroit_relocate.py:288-402)."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
     from oracle.adroit_env import OracleAdroitRelocateEnv
-
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
 
     m = load_model("adroit_relocate")
     assert m.nv == 36 and m.nu == 30
-    env = pkg.make_vec("AdroitHandRelocate-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("AdroitHandRelocate-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.single_observation_space.shape == (39,) and env.single_action_space.shape == (30,)
     orc = OracleAdroitRelocateEnv(m, noslip=False)
     obs, _ = env.reset(seed=4)
@@ -363,14 +353,10 @@ def test_adroit_relocate_env_matches_oracle():
 def test_adroit_pen_env_matches_oracle():
     """AdroitHandPen-v2 (30 dofs): the pen is a cylinder (portal-refinement collider) and the static target pen's
     quaternion is per-env state (two Euler draws per reset); obs 45, dense / sparse reward (adroit_pen.py:288-430)."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
     from oracle.adroit_env import OracleAdroitPenEnv
 
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
     m = load_model("adroit_pen")
-    env = pkg.make_vec("AdroitHandPen-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("AdroitHandPen-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.single_observation_space.shape == (45,) and env.single_action_space.shape == (24,)
     orc = OracleAdroitPenEnv(m, noslip=False)
     obs, _ = env.reset(seed=4)
@@ -399,7 +385,7 @@ def test_adroit_pen_env_matches_oracle():
         assert d.max() < 2e-2                               # fp32 vs fp64 portal normals (1e-4) torque the light pen
         assert abs(float(r[0]) - orr) < 2e-4 and bool(info["success"][0]) == bool(oi["success"])
     assert np.median(errs) < 2e-3
-    envs = pkg.make_vec("AdroitHandPenSparse-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    envs = pkg.make_vec("AdroitHandPenSparse-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     envs.reset(seed=4)
     _, r, *_ = envs.step(np.zeros((1, 24), dtype=np.float32))
     assert float(r[0]) == pytest.approx(-0.1)
@@ -409,15 +395,11 @@ def test_adroit_pen_env_matches_oracle():
 def test_adroit_door_env_matches_oracle():
     """AdroitHandDoor-v2 (30 dofs, 278 candidate geom pairs -> two-byte broad-phase candidates; cylinder door posts and
     latch through the portal-refinement collider; per-env door frame position) (adroit_door.py:279-402)."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
     from oracle.adroit_env import OracleAdroitDoorEnv
-
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
 
     m = load_model("adroit_door")
     assert len(m.pair_geom1) > 255
-    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy")
     assert env.single_observation_space.shape == (39,) and env.single_action_space.shape == (28,)
     orc = OracleAdroitDoorEnv(m, noslip=False)
     obs, _ = env.reset(seed=4)
@@ -448,12 +430,8 @@ def test_adroit_door_env_matches_oracle():
 
 def test_adroit_reset_honours_initial_state_dict():
     """adroit_hammer.py:359-370: reset(options={"initial_state_dict": ...}) = ordinary reset, then set_env_state."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
 
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
-    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=2, backend_factory=AdroitHostBackend, rng_mode="numpy")
+    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=2, backend_factory=HostSimBackend, rng_mode="numpy")
     obs0, _ = env.reset(seed=3)
     sd = env.get_env_state()
     q = sd["qpos"][0].clone()

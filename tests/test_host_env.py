@@ -235,12 +235,8 @@ def test_auto_recover_detects_and_resets_bad_states():
 def test_auto_recover_on_other_families():
     """The scan keeps what an episode drew: the Adroit door's frame position (per-env model pose) survives a recovery."""
     import gymnasium_robotics_b200 as pkg
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
 
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
-    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=2, backend_factory=AdroitHostBackend, rng_mode="numpy", auto_recover=True)
+    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=2, backend_factory=HostSimBackend, rng_mode="numpy", auto_recover=True)
     env.reset(seed=1)
     frame = env.get_env_state()["door_body_pos"].clone()
     st = env.backend.state

@@ -13,11 +13,11 @@ from tests.hostsim_backend import HostSimBackend
 
 
 class TwoLevel(HostSimBackend):
-    REF, FLAVOR = KITCHEN_REF_POINT, "kitchen_groups"
+    FLAVOR = "kitchen_groups"
 
 
 class FlatScan(HostSimBackend):
-    REF, FLAVOR = KITCHEN_REF_POINT, "kitchen_flat"
+    FLAVOR = "kitchen_flat"
 
 
 def test_group_table_covers_every_pair_once():

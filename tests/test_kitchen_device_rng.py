@@ -1,18 +1,16 @@
 """FrankaKitchen rng_mode="device" on the kitchen-flavor host emulation of the kernel source: the observation noise drawn by
 kitchen_observe (csrc/fetch_task.cuh) is Philox4x32-10 over (seed; global env index, episode, step), bit for bit the restatement
 below, uniform per entry, and a pure function of the state, so that get_state / set_state checkpoint a Kitchen env."""
-import ctypes
-import types
+import functools
 
 import numpy as np
 import pytest
 import torch
 from scipy import stats
 
-from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT, KitchenVectorEnv
+from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
 from gymnasium_robotics_b200.models import load_model
 from tests import hostsim
-from tests.hostsim import kitchen_noise
 from tests.hostsim_backend import HostSimBackend
 
 NOBS = 59
@@ -20,10 +18,7 @@ TAG = 0x0B5E
 
 
 def _philox():
-    L = hostsim.lib(wide=False)
-    L.hostsim_philox4x32_10.argtypes = [ctypes.c_void_p] * 3
-    L.hostsim_philox4x32_10.restype = None
-    return L.hostsim_philox4x32_10
+    return hostsim.lib(wide=False).hostsim_philox4x32_10
 
 
 def restated_uniforms(seed, env, episode, t):
@@ -47,66 +42,12 @@ def restated_obs(clean, scale, seed, env, episode, t):
     return (np.asarray(clean, dtype=np.float32) + noise).astype(np.float32)
 
 
-class NoiseHostBackend(HostSimBackend):
-    """HostSimBackend with b200sim_set_obs_noise: every env call goes through hostsim_kitchen_env_step (tests/hostsim/kitchen_noise.cpp)
-    with the env's noise key as the step kernel builds it (global index, episode counter, step counter after the call), or with no
-    key while the noise is off."""
-    REF = KITCHEN_REF_POINT
-    FLAVOR = "kitchen"
-    noise = None
-
-    def __init__(self, model, eq_data, task, num_envs, device):
-        super().__init__(model, eq_data, task, num_envs, device)
-        self._L = kitchen_noise.lib(self.FLAVOR)
-        blob, ref = model.to_blob(), np.asarray(self.REF, dtype=np.float32)
-        self._h = self._L.hostsim_create(blob, len(blob), None, ref.ctypes.data, -1, 0)
-        assert self._h
-        self.sim._L.hostsim_destroy(self.sim._h)   # the plain emulation's handle: this backend steps through its own library
-        self.sim = types.SimpleNamespace(env_step=self._env_step, _L=self._L)
-        self._env_iter = None
-
-    def close(self):
-        if self._h:
-            self._L.hostsim_destroy(self._h)
-            self._h = None
-
-    def set_obs_noise(self, scale, seed, env_offset, episode):
-        self.noise = None if scale is None else (scale.numpy(), int(seed) & 0xFFFFFFFFFFFFFFFF, int(env_offset), episode)
-
-    def _env_step(self, task, mode, nraw, st, action, nobs, ngoal):
-        i = next(self._env_iter)
-        obs, ag, dg = np.zeros(nobs, np.float32), np.zeros(ngoal, np.float32), np.zeros(ngoal, np.float32)
-        rew, suc = np.zeros(1, np.float32), np.zeros(1, np.float32)
-        a = np.zeros(32, np.float32)
-        a[:len(action)] = action
-        scale, seed, offset, episode = self.noise if self.noise is not None else (None, 0, 0, None)
-        ep = int(episode[i]) if episode is not None else 0
-        step = int(self.elapsed[i]) + (1 if mode == 0 else 0)
-        it = self._L.hostsim_kitchen_env_step(self._h, ctypes.byref(task), mode, nraw, scale.ctypes.data if scale is not None else None, seed,
-                                              offset + i, ep, step, st.ctypes.data, a.ctypes.data, obs.ctypes.data, ag.ctypes.data,
-                                              dg.ctypes.data, rew.ctypes.data, suc.ctypes.data)
-        return obs, ag, dg, float(rew[0]), float(suc[0]), it
-
-    def _run(self, mode, nraw, actions, mask, out, info=None):
-        # the envs in the order HostSimBackend._run steps them: the noise key needs each call's env index
-        self._env_iter = iter([i for i in range(self.num_envs) if mask is None or bool(mask[i])])
-        super()._run(mode, nraw, actions, mask, out, info)
-
-
-class NoiseHostBackendGroups(NoiseHostBackend):
-    FLAVOR = "kitchen_groups"
-
-
-class NoiseHostBackendHull(NoiseHostBackend):
-    FLAVOR = "kitchen_hull"
-
-
 @pytest.fixture(scope="module")
 def model():
     return load_model("franka_kitchen")
 
 
-def _make(model, n, backend=NoiseHostBackend, **kw):
+def _make(model, n, backend=functools.partial(HostSimBackend, flavor="kitchen"), **kw):   # the flat-scan build
     kw.setdefault("rng_mode", "device")
     return KitchenVectorEnv(num_envs=n, backend_factory=backend, device="cpu", model=model, **kw)
 
@@ -133,10 +74,8 @@ def _check_noise(env, noisy, elapsed=None):
 
 
 def test_known_answers_match_the_restatement():
-    L = kitchen_noise.lib("kitchen")
-    out = np.zeros(NOBS, np.float32)
     for seed, env, episode, t in ((0, 0, 0, 0), (7, 3, 1, 0), (2**40 + 12345, 2047, 9, 279), (-3, 1 << 20, 123456, (1 << 28) - 1), (2**64 - 1, 5, 2, 17)):
-        L.hostsim_kitchen_noise(seed & 0xFFFFFFFFFFFFFFFF, env, episode, t, out.ctypes.data)
+        out = hostsim.kitchen_noise(seed, env, episode, t)
         want = restated_uniforms(seed, env, episode, t)
         assert np.array_equal(out.view(np.int32), want.view(np.int32)), (seed, env, episode, t)
         assert out.min() >= -1.0 and out.max() < 1.0
@@ -191,11 +130,10 @@ def test_noise_after_same_step_autoreset(model):
 
 
 def test_noise_is_uniform_per_entry_and_independent():
-    L = kitchen_noise.lib("kitchen")
     n = 4000
     u = np.zeros((n, NOBS), np.float32)
     for k in range(n):
-        L.hostsim_kitchen_noise(77, k % 500, 1 + k // 2000, (k // 500) % 4 * 70 + 3, u[k].ctypes.data)
+        u[k] = hostsim.kitchen_noise(77, k % 500, 1 + k // 2000, (k // 500) % 4 * 70 + 3)
     for j in range(NOBS):
         assert stats.kstest(u[:, j], "uniform", args=(-1.0, 2.0)).pvalue > 1e-4, j
     # robot entries (18) against object entries (41): no correlation beyond sampling noise
@@ -207,11 +145,10 @@ def test_noise_is_uniform_per_entry_and_independent():
 def test_scaled_noise_is_uniform_on_the_scale(model):
     env = _make(model, 1)
     scale = env._noise_scale.numpy()
-    L = kitchen_noise.lib("kitchen")
     n = 2000
     u = np.zeros((n, NOBS), np.float32)
     for k in range(n):
-        L.hostsim_kitchen_noise(5, k, 1, 0, u[k].ctypes.data)
+        u[k] = hostsim.kitchen_noise(5, k, 1, 0)
     noise = u * scale
     for j in (0, 8, 9, 17, 18, 38, 39, 58):
         assert np.abs(noise[:, j]).max() <= scale[j]
@@ -275,10 +212,10 @@ def test_set_state_still_raises_with_host_noise(model, rng_mode):
 
 @pytest.mark.parametrize("kind", ["flat", "groups", "hull"])
 def test_device_mode_builds_for_every_kitchen_build(kind):
-    backend = {"flat": NoiseHostBackend, "groups": NoiseHostBackendGroups, "hull": NoiseHostBackendHull}[kind]
     kw = {"flat": dict(broadphase="flat"), "groups": dict(broadphase="groups"), "hull": dict(mesh_collision="hull")}[kind]
     m = load_model("franka_kitchen_hull" if kind == "hull" else "franka_kitchen")
-    env = _make(m, 2, backend=backend, **kw)
+    env = _make(m, 2, backend=HostSimBackend, **kw)
+    assert env.backend.flavor == {"flat": "kitchen", "groups": "kitchen_groups", "hull": "kitchen_hull"}[kind]
     obs, info = env.reset(seed=8)
     assert info["tasks_to_complete"].all()
     _check_noise(env, obs["observation"])

@@ -6,14 +6,13 @@ import numpy as np
 import pytest
 import torch
 
-from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT, KitchenVectorEnv
+from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
 from gymnasium_robotics_b200.models import load_model
 from oracle.kitchen_env import OracleKitchenEnv
 from tests.hostsim_backend import HostSimBackend
 
 
 class KitchenHostBackend(HostSimBackend):
-    REF = KITCHEN_REF_POINT
     FLAVOR = "kitchen"
 
 

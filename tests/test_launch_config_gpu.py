@@ -16,7 +16,7 @@ import pytest
 import torch
 
 import gymnasium_robotics_b200 as pkg
-from gymnasium_robotics_b200.fetch import REF_POINT, welded_eq_data
+from gymnasium_robotics_b200.fetch import welded_eq_data
 
 pytestmark = pytest.mark.gpu
 
@@ -84,7 +84,7 @@ def _create(env, eq, n, wpb, mp):
     if hasattr(env, "broadphase"):
         mp.setenv("B200SIM_KITCHEN_GROUPS", "1" if env.broadphase == "groups" else "0")
     L, blob = env.backend.L, env.model.to_blob()
-    ref = np.asarray(getattr(env.backend, "REF", REF_POINT), dtype=np.float32)
+    ref = np.asarray(env.backend.ref, dtype=np.float32)
     eq = np.ascontiguousarray(eq, dtype=np.float64)
     h = ctypes.c_void_p()
     rc = L.b200sim_create(blob, len(blob), eq.ctypes.data if eq.size else None, ref.ctypes.data, ctypes.byref(env.task), n,

@@ -14,8 +14,7 @@ from gymnasium_robotics_b200.maze import NOISE, SUCCESS_RADIUS
 from oracle.ant_maze_env import OracleAntMazeEnv
 from oracle.maze import MazeResetLogic
 from oracle.point_maze_env import OraclePointMazeEnv
-from tests.hostsim import maze_goal
-from tests.hostsim.maze_goal import GoalUpdateHostBackend
+from tests import hostsim
 from tests.hostsim_backend import HostSimBackend
 from tests.test_reset_device import M32, philox4x32_10, py_maze_draw, u01
 
@@ -86,7 +85,12 @@ class GoalOraclePointMaze(_UpdateGoal, OraclePointMazeEnv):
 
 
 # ---------------------------------------------------------------------------------------------- helpers
-def _make(env_id="PointMaze_Large-v3", n=4, backend=GoalUpdateHostBackend, **kw):
+class NoHooks(HostSimBackend):
+    """A backend without the handle's optional hooks."""
+    set_goal_update = set_goal_redraw = set_ant_info = set_obs_noise = None
+
+
+def _make(env_id="PointMaze_Large-v3", n=4, backend=HostSimBackend, **kw):
     kw.setdefault("rng_mode", "device")
     kw.setdefault("reset_target", True)
     return pkg.make_vec(env_id, num_envs=n, backend_factory=backend, **kw)
@@ -124,17 +128,17 @@ def test_known_answers_and_edge_keys():
             for ach in ([0.5, 1.5], [0.7, 1.6], [10.0, 10.0]):
                 goal = np.asarray(ach, dtype=f32) + f32(0.2)
                 want = py_goal_update(goal_xy * f32(scaling), scaling, NOISE, SUCCESS_RADIUS, seed, env, ep, step, ach, goal)
-                got = maze_goal.goal_update(goal_xy * f32(scaling), scaling, NOISE, SUCCESS_RADIUS, seed, env, ep, step, ach, goal)
+                got = hostsim.goal_update(goal_xy * f32(scaling), scaling, NOISE, SUCCESS_RADIUS, seed, env, ep, step, ach, goal)
                 assert got[1] == want[1] >= 1 and np.array_equal(got[0], want[0]), (seed, env, ep, step, scaling, ach)
     # no update when the achieved position is outside the radius
-    g, n = maze_goal.goal_update(goal_xy, 1.0, NOISE, SUCCESS_RADIUS, 1, 2, 3, 4, [0.0, 0.0], [0.46, 0.0])
+    g, n = hostsim.goal_update(goal_xy, 1.0, NOISE, SUCCESS_RADIUS, 1, 2, 3, 4, [0.0, 0.0], [0.46, 0.0])
     assert n == 0 and np.array_equal(g, f32([0.46, 0.0]))
     # a key whose first candidates are rejected: the agent sits on one of two goal cells (scaling 1: its noise box lies in the disc)
     two = np.array([[0.0, 0.0], [3.0, 0.0]], dtype=f32)
     found = 0
     for step in range(200):
         want = py_goal_update(two, 1.0, NOISE, SUCCESS_RADIUS, 99, 5, 1, step, [0.0, 0.0], [0.0, 0.0])
-        got = maze_goal.goal_update(two, 1.0, NOISE, SUCCESS_RADIUS, 99, 5, 1, step, [0.0, 0.0], [0.0, 0.0])
+        got = hostsim.goal_update(two, 1.0, NOISE, SUCCESS_RADIUS, 99, 5, 1, step, [0.0, 0.0], [0.0, 0.0])
         assert got[1] == want[1] and np.array_equal(got[0], want[0])
         assert abs(float(got[0][0]) - 3.0) <= 0.25 and _dist_host([0, 0], got[0]) > f32(SUCCESS_RADIUS)
         found = max(found, got[1])
@@ -147,7 +151,7 @@ def test_candidates_are_uniform_over_cells_and_noise():
     far = [-100.0, -100.0]
     cells, noise = [], []
     for k in range(14000):
-        g, n = maze_goal.goal_update(goal_xy, 4.0, NOISE, SUCCESS_RADIUS, 2024, k % 500, k // 500, 17, far, far)
+        g, n = hostsim.goal_update(goal_xy, 4.0, NOISE, SUCCESS_RADIUS, 2024, k % 500, k // 500, 17, far, far)
         assert n == 1
         c = int(np.rint(g[0] / 4.0))
         cells.append(c)
@@ -233,7 +237,7 @@ def test_gates_leave_goals_and_launches_as_today(case):
     elif case == "numpy_mode":
         kw["rng_mode"] = "numpy"
     counts = []
-    for backend in (GoalUpdateHostBackend, HostSimBackend):
+    for backend in (HostSimBackend, NoHooks):
         env = _make(env_id, n=3, backend=backend, **kw)
         obs, _ = env.reset(seed=8)
         g0 = _goals(env).clone()
@@ -242,7 +246,7 @@ def test_gates_leave_goals_and_launches_as_today(case):
         assert info["success"].all()
         if case != "numpy_mode":
             assert torch.equal(_goals(env), g0)          # no update in any mode
-        assert env.backend.goal_args is None if backend is GoalUpdateHostBackend else True
+        assert env.backend.goal_args is None if backend is HostSimBackend else True
         counts.append(env.backend.launches)
         env.close()
     assert counts[0] == counts[1]
@@ -302,8 +306,8 @@ def test_options_resets_advance_the_episode_of_the_update_stream():
 
 def test_backend_without_the_update_is_refused_in_device_mode():
     with pytest.raises(NotImplementedError):
-        _make(n=2, backend=HostSimBackend)
-    _make(n=2, backend=HostSimBackend, reset_target=False).close()
+        _make(n=2, backend=NoHooks)
+    _make(n=2, backend=NoHooks, reset_target=False).close()
 
 
 # ---------------------------------------------------------------------------------------------- numpy mode against the oracle

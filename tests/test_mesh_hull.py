@@ -68,13 +68,10 @@ def test_box_proxy_models_are_refused_by_nothing_and_mesh_models_by_the_plain_bu
 def test_kitchen_hull_env_tracks_the_oracle_env():
     import torch
 
-    from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT, KitchenVectorEnv
+    from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
     from gymnasium_robotics_b200.models import load_model
     from oracle.kitchen_env import OracleKitchenEnv
     from tests.hostsim_backend import HostSimBackend
-
-    class HullBackend(HostSimBackend):
-        REF, FLAVOR = KITCHEN_REF_POINT, "kitchen_hull"
 
     model = load_model("franka_kitchen_hull")
     gh = np.asarray(model.geom_hull).reshape(-1, 2)
@@ -84,7 +81,7 @@ def test_kitchen_hull_env_tracks_the_oracle_env():
         v = model.hull_vert[gh[g, 0]: gh[g, 0] + gh[g, 1]]
         assert np.all(np.abs(v) <= model.geom_size[g] + 1e-9) and np.allclose(np.abs(v).max(axis=0), model.geom_size[g], atol=1e-9)
     n, seed = 2, 31
-    env = KitchenVectorEnv(num_envs=n, backend_factory=HullBackend, device="cpu", rng_mode="numpy", model=model, mesh_collision="hull")
+    env = KitchenVectorEnv(num_envs=n, backend_factory=HostSimBackend, device="cpu", rng_mode="numpy", model=model, mesh_collision="hull")
     obs, _ = env.reset(seed=seed)
     orcs = [OracleKitchenEnv(model) for _ in range(n)]
     for i, o in enumerate(orcs):
@@ -105,16 +102,13 @@ def test_kitchen_hull_env_tracks_the_oracle_env():
 def test_kitchen_hull_contact_phase_matches_the_oracle():
     """The contact case: a constant action drives the arm until a link's hull touches the kitchen (oracle: a contact with a MESH geom from
     env-step 7 on); the env on the hull emulation keeps tracking the oracle env through the touch."""
-    from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT, KitchenVectorEnv
+    from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
     from gymnasium_robotics_b200.models import load_model
     from oracle.kitchen_env import OracleKitchenEnv
     from tests.hostsim_backend import HostSimBackend
 
-    class HullBackend(HostSimBackend):
-        REF, FLAVOR = KITCHEN_REF_POINT, "kitchen_hull"
-
     model = load_model("franka_kitchen_hull")
-    env = KitchenVectorEnv(num_envs=1, backend_factory=HullBackend, device="cpu", rng_mode="numpy", model=model, mesh_collision="hull")
+    env = KitchenVectorEnv(num_envs=1, backend_factory=HostSimBackend, device="cpu", rng_mode="numpy", model=model, mesh_collision="hull")
     env.reset(seed=1)
     orc = OracleKitchenEnv(model)
     orc.reset(seed=1)

@@ -81,9 +81,6 @@ def py_fetch_draw(p, seed, env, episode):
 
 def c_fetch_record(p, seed, env, episode, rest, st_qpos, st_goal):
     L = hostsim.lib()
-    L.hostsim_fetch_reset_record.argtypes = [ctypes.c_void_p, ctypes.c_ulonglong, ctypes.c_uint, ctypes.c_uint, ctypes.c_void_p, ctypes.c_int,
-                                             ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    L.hostsim_fetch_reset_record.restype = None
     rec = np.zeros_like(rest)
     L.hostsim_fetch_reset_record(ctypes.byref(p), seed, env, episode, rest.ctypes.data, len(rest), st_qpos, st_goal, rec.ctypes.data)
     return rec
@@ -182,9 +179,6 @@ def test_uniform_slot_reset_against_python():
     from gymnasium_robotics_b200._lib import UniformResetC
 
     L = hostsim.lib()
-    L.hostsim_uniform_reset_record.argtypes = [ctypes.c_void_p, ctypes.c_ulonglong, ctypes.c_uint, ctypes.c_uint, ctypes.c_void_p, ctypes.c_int,
-                                               ctypes.c_void_p]
-    L.hostsim_uniform_reset_record.restype = None
     p = UniformResetC()
     slots, lo, hi = [3, 40, 41, 7, 12, 13], [-0.15, -0.15, -0.2, 0.1, 0.0, 5.0], [0.15, 0.3, 0.2, 0.25, 1.0, 5.0]
     p.n, p.quat_slot = 6, -1
@@ -212,18 +206,13 @@ def test_uniform_slot_reset_against_python():
 
 def test_adroit_door_env_with_in_kernel_resets():
     """adroit_door.py:359-371: the frame position is three uniform draws per episode; everything else is the model's rest state."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
-
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
-    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=3, backend_factory=AdroitHostBackend, rng_mode="device", max_episode_steps=2)
+    env = pkg.make_vec("AdroitHandDoor-v2", num_envs=3, backend_factory=HostSimBackend, rng_mode="device", max_episode_steps=2)
     o, _ = env.reset(seed=5)
     s = env.get_env_state()
     pos = s["door_body_pos"].numpy()
     assert ((pos >= [-0.3, 0.25, 0.252]) & (pos <= [-0.2, 0.35, 0.35])).all() and len({tuple(r) for r in pos.round(6).tolist()}) == 3
     assert torch.equal(s["qpos"], env.init_qpos.expand(3, -1)) and torch.count_nonzero(s["qvel"]) == 0
-    env2 = pkg.make_vec("AdroitHandDoor-v2", num_envs=3, backend_factory=AdroitHostBackend, rng_mode="device")
+    env2 = pkg.make_vec("AdroitHandDoor-v2", num_envs=3, backend_factory=HostSimBackend, rng_mode="device")
     o2, _ = env2.reset(seed=5)
     assert torch.equal(o, o2)
     for _ in range(3):     # TimeLimit 2: the third call is the next-step reset with new draws
@@ -232,7 +221,7 @@ def test_adroit_door_env_with_in_kernel_resets():
     # the Pen's target orientation: euler2quat of two draws (adroit_pen.py:379-384), against utils/rotations.py's restatement
     from gymnasium_robotics_b200 import rotations
 
-    pen = pkg.make_vec("AdroitHandPen-v2", num_envs=4, backend_factory=AdroitHostBackend, rng_mode="device")
+    pen = pkg.make_vec("AdroitHandPen-v2", num_envs=4, backend_factory=HostSimBackend, rng_mode="device")
     pen.reset(seed=9)
     quat = pen.get_env_state()["desired_orien"].numpy()
     for i in range(4):
@@ -300,15 +289,12 @@ def test_hand_env_with_in_kernel_resets():
     """manipulate.py:154-279 in rng_mode="device": start pose (z-rotation / parallel / xyz offset, position noise), settle with the
     on-palm retry, goal from the settled pose -- checked against the reference's formulas on the same Philox numbers."""
     from gymnasium_robotics_b200 import rotations
-    from gymnasium_robotics_b200.hand import HAND_REF_POINT, TARGET_POSITION_RANGE
-
-    class HandHostBackend(HostSimBackend):
-        REF = HAND_REF_POINT
+    from gymnasium_robotics_b200.hand import TARGET_POSITION_RANGE
 
     f = np.float32
     for env_id, rot in (("HandManipulateBlockRotateZ-v1", "z"), ("HandManipulateBlockRotateParallel-v1", "parallel"),
                         ("HandManipulateBlockFull-v1", "xyz")):
-        env = pkg.make_vec(env_id, num_envs=2, backend_factory=HandHostBackend, rng_mode="device")
+        env = pkg.make_vec(env_id, num_envs=2, backend_factory=HostSimBackend, rng_mode="device")
         o, _ = env.reset(seed=13)
         assert env.reset_attempts >= 1 and int(env._episode.min()) == 1
         st, _ = env.get_state()
@@ -335,7 +321,7 @@ def test_hand_env_with_in_kernel_resets():
                 assert np.abs(goal[i, :3] - (obj[i, :3] + off)).max() < 2e-6
             else:
                 assert np.abs(goal[i, :3] - obj[i, :3]).max() < 1e-7          # "ignore": the goal position is the settled object's
-        env2 = pkg.make_vec(env_id, num_envs=2, backend_factory=HandHostBackend, rng_mode="device")
+        env2 = pkg.make_vec(env_id, num_envs=2, backend_factory=HostSimBackend, rng_mode="device")
         o2, _ = env2.reset(seed=13)
         assert torch.equal(o["observation"], o2["observation"]) and torch.equal(o["desired_goal"], o2["desired_goal"])
 
@@ -346,9 +332,6 @@ def test_hand_start_pose_draw():
     from gymnasium_robotics_b200._lib import HandResetC
 
     L = hostsim.lib()
-    L.hostsim_hand_pose_record.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_ulonglong, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint,
-                                           ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    L.hostsim_hand_pose_record.restype = None
     par = np.array(rotations.parallel_quats(), dtype=np.float32)
     p = HandResetC()
     p.obj_qadr, p.randomize_rotation, p.randomize_position = 24, 1, 1
@@ -385,12 +368,7 @@ def test_hand_start_pose_draw():
 
 def test_hand_reach_goal_draw():
     """reach.py:95-121 on the generator's numbers: thumb + one of four fingers meet near the palm; 10 % keep the initial tips."""
-    from gymnasium_robotics_b200.hand import HAND_REF_POINT
-
-    class HandHostBackend(HostSimBackend):
-        REF = HAND_REF_POINT
-
-    env = pkg.make_vec("HandReach-v3", num_envs=40, backend_factory=HandHostBackend, rng_mode="device")
+    env = pkg.make_vec("HandReach-v3", num_envs=40, backend_factory=HostSimBackend, rng_mode="device")
     o, _ = env.reset(seed=6)
     goals = o["desired_goal"].numpy().reshape(40, 5, 3)
     init = env.initial_goal.numpy().reshape(5, 3)

@@ -102,12 +102,7 @@ def test_recorder_matches_a_plain_rollout():
 
 def test_recorder_on_flat_observations():
     """Adroit envs return a flat observation tensor and `info["success"]` (adroit_hammer.py:291-357)."""
-    from gymnasium_robotics_b200.adroit import ADROIT_REF_POINT
-
-    class AdroitHostBackend(HostSimBackend):
-        REF = ADROIT_REF_POINT
-
-    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=AdroitHostBackend, rng_mode="numpy", max_episode_steps=3)
+    env = pkg.make_vec("AdroitHandHammer-v2", num_envs=1, backend_factory=HostSimBackend, rng_mode="numpy", max_episode_steps=3)
     rec = RolloutRecorder(env, capacity_steps=8)
     rec.reset(seed=0)
     for _ in range(5):

@@ -1,6 +1,8 @@
 """Random-action soak of the kernel source on the CPU emulation: several env families, aggressive actions (every fourth
 step saturated), TimeLimit + same-step autoreset.  Observations must stay finite and capacity overflow may only show up as
 flags in the info word (the counted-but-unwritten contact record was found by exactly this kind of run at scale)."""
+import functools
+
 import numpy as np
 import pytest
 import torch
@@ -18,11 +20,9 @@ CASES = [("FetchPickAndPlace-v4", REF_POINT), ("FetchSlide-v4", REF_POINT), ("Ha
 
 @pytest.mark.parametrize("env_id,ref", CASES)
 def test_random_action_soak_stays_finite(env_id, ref):
-    class B(HostSimBackend):
-        REF = ref
-
     n, steps = 6, 36
-    env = pkg.make_vec(env_id, num_envs=n, backend_factory=B, rng_mode="torch", autoreset_mode="same_step", max_episode_steps=15)
+    env = pkg.make_vec(env_id, num_envs=n, backend_factory=HostSimBackend, rng_mode="torch", autoreset_mode="same_step", max_episode_steps=15)
+    assert tuple(env.backend.sim.ref) == pytest.approx(ref)
     env.reset(seed=0)
     g = torch.Generator().manual_seed(7)
     for k in range(steps):
@@ -41,12 +41,8 @@ def test_kitchen_soak_with_the_two_level_broad_phase(flavor):
     """FrankaKitchen-v1 on the kitchen-flavor emulation (29 dofs, 3 708 pairs in 1 010 groups): saturated actions sweep the arm
     through the scene; no capacity flag at all (a longer run of 5 600 env-steps saw none either, up to 57 candidates)."""
     from gymnasium_robotics_b200.kitchen import KitchenVectorEnv
-    from gymnasium_robotics_b200.kitchen import KITCHEN_REF_POINT
 
-    class KitchenHostBackend(HostSimBackend):
-        REF, FLAVOR = KITCHEN_REF_POINT, flavor
-
-    env = KitchenVectorEnv(num_envs=4, backend_factory=KitchenHostBackend, device="cpu", rng_mode="torch", autoreset_mode="same_step",
+    env = KitchenVectorEnv(num_envs=4, backend_factory=functools.partial(HostSimBackend, flavor=flavor), device="cpu", rng_mode="torch", autoreset_mode="same_step",
                            max_episode_steps=25)
     env.reset(seed=0)
     g = torch.Generator().manual_seed(3)

@@ -1,10 +1,13 @@
 """The gymnasium vector-env contract of every env class, on the host emulation: the three autoreset modes (NEXT_STEP, SAME_STEP,
 disabled) of the one state machine in vector.py, the info keys each family reports, and the construction checks every family
 shares (rng_mode, auto_recover, obs_dtype)."""
+import functools
+
 import numpy as np
 import pytest
 import torch
 
+from tests.hostsim_backend import HostSimBackend
 from tests.test_api_conformance import _leaves, _make
 
 T = 2   # max_episode_steps: the second step truncates
@@ -118,9 +121,14 @@ def test_unknown_rng_mode_is_refused(case):
         _env(case, rng_mode="philox")
 
 
+class NoHooks(HostSimBackend):
+    """A backend without the handle's optional hooks."""
+    set_goal_update = set_goal_redraw = set_ant_info = set_obs_noise = None
+
+
 def test_kitchen_has_no_device_rng():
     with pytest.raises(NotImplementedError, match="rng_mode='device'"):
-        _env("FrankaKitchen-v1", rng_mode="device")
+        _env("FrankaKitchen-v1", rng_mode="device", backend_factory=functools.partial(NoHooks, flavor="kitchen"))
 
 
 @pytest.mark.parametrize("case", ["AntMaze_UMaze-v5/continuing", "PointMaze_UMaze-v3", "FrankaKitchen-v1"])

@@ -3,6 +3,8 @@
 lines nvcc compiles for the device -- shuffle reductions, exclusive scans, ballots, the register-resident (and bordered) Cholesky
 with its shared-memory column broadcast, the two-level broad phase -- and run them on 32 lock-step fibers (tests/hostsim/hostwarp.h).
 Here one env-step of every kernel family from identical state records: 32-lane execution against the 1-lane execution."""
+import functools
+
 import numpy as np
 import pytest
 import torch
@@ -30,12 +32,7 @@ CASES = [("FetchPickAndPlace-v4", REF_POINT, None, "warp", 4, 2e-4),
 
 @pytest.mark.parametrize("env_id,ref,flavor1,flavor32,warm,tol", CASES)
 def test_32_lane_execution_matches_1_lane_execution(env_id, ref, flavor1, flavor32, warm, tol):
-    class W1(HostSimBackend):
-        REF, FLAVOR = ref, flavor1
-
-    class W32(HostSimBackend):
-        REF, FLAVOR = ref, flavor32
-
+    W1, W32 = (functools.partial(HostSimBackend, flavor=f) for f in (flavor1, flavor32))
     kw = dict(experimental=True) if env_id.startswith("Franka") else {}
     env = pkg.make_vec(env_id, num_envs=1, backend_factory=W1, rng_mode="numpy", **kw)
     env.reset(seed=3)
@@ -44,6 +41,7 @@ def test_32_lane_execution_matches_1_lane_execution(env_id, ref, flavor1, flavor
     for _ in range(warm):
         env.step(rng.uniform(-1, 1, size=(1, nact)).astype(np.float32))
     b1 = env.backend
+    assert tuple(b1.sim.ref) == pytest.approx(ref)
     eq = welded_eq_data(env.model) if env.model.nmocap > 0 else np.zeros((0, 11))
     b32 = W32(env.model, eq, env.task, 1, "cpu")
     assert b32.layout == b1.layout
@@ -113,12 +111,9 @@ def test_kitchen_env_tracks_the_oracle_on_the_32_lane_emulation(flavor):
     from gymnasium_robotics_b200.models import load_model
     from oracle.kitchen_env import OracleKitchenEnv
 
-    class B(HostSimBackend):
-        REF, FLAVOR = KITCHEN_REF_POINT, flavor
-
     m = load_model("franka_kitchen")
     n, seed = 2, 21
-    env = KitchenVectorEnv(num_envs=n, backend_factory=B, device="cpu", rng_mode="numpy", model=m)
+    env = KitchenVectorEnv(num_envs=n, backend_factory=functools.partial(HostSimBackend, flavor=flavor), device="cpu", rng_mode="numpy", model=m)
     obs, _ = env.reset(seed=seed)
     orcs = [OracleKitchenEnv(m) for _ in range(n)]
     for i, o in enumerate(orcs):

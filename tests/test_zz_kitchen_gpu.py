@@ -11,11 +11,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _backend(n):
-    from gymnasium_robotics_b200.kitchen import _KitchenBackend, make_kitchen_task
+    from gymnasium_robotics_b200.fetch import CudaBackend
+    from gymnasium_robotics_b200.kitchen import make_kitchen_task
     from gymnasium_robotics_b200.models import load_model
 
     m = load_model("franka_kitchen")
-    return m, _KitchenBackend(m, np.zeros((0, 11)), make_kitchen_task(m), n, "cuda:0")
+    return m, CudaBackend(m, np.zeros((0, 11)), make_kitchen_task(m), n, "cuda:0")
 
 
 from tests.parity_util import check_envelope
