@@ -159,7 +159,6 @@ class _AdroitVectorEnv(VectorEnv):
                     p.slot[k] = sl[field].start + off
                 p.lo[k], p.hi[k] = lo, hi
             self._dev_reset = (p, self._rest)
-            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         every = self._reset_all
         p, rest = self._dev_reset
         self.backend.reset_uniform(None if every else mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)
@@ -208,6 +207,8 @@ class _AdroitVectorEnv(VectorEnv):
     def reset(self, *, seed=None, options=None):
         """adroit_hammer.py:359-370 (and the siblings): `options={"initial_state_dict": {...}}` sets the state after the
         ordinary reset through `set_env_state` (entries [width] for every env or [num_envs, width])."""
+        if options is not None and "initial_state_dict" in options and "reset_mask" in options:
+            raise ValueError("initial_state_dict sets the state of every env: it does not combine with reset_mask")
         obs, info = super().reset(seed=seed, options=options)
         if options is not None and "initial_state_dict" in options:
             obs = self._cast_obs(self.set_env_state(options["initial_state_dict"]))

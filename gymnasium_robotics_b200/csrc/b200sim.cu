@@ -44,36 +44,39 @@ __global__ void reward_kernel(const float* __restrict__ ag, const float* __restr
 }
 
 // in-kernel reset draw (reset_sample.cuh): one thread per env writes its state record; the refresh launch that follows does
-// mj_forward + _get_obs.  32 consecutive threads write 32 consecutive records word by word (stride ~ 60 words: each record is
+// mj_forward + _get_obs.  Every draw kernel keys env i's Philox stream with keys[i] when the handle has a key table
+// (b200sim_set_env_keys), else with the `seed` argument.  32 consecutive threads write 32 consecutive records word by word (stride ~ 60 words: each record is
 // a few 128-byte lines, touched once per episode).
-__global__ void fetch_reset_kernel(b200sim_fetch_reset_t p, unsigned long long seed, int env_offset, int N, const unsigned char* __restrict__ mask,
+__global__ void fetch_reset_kernel(b200sim_fetch_reset_t p, unsigned long long seed, const unsigned long long* __restrict__ keys, int env_offset, int N,
+                                   const unsigned char* __restrict__ mask,
                                    const float* __restrict__ rest, int stride, int st_qpos, int st_goal, float* __restrict__ state,
                                    int* __restrict__ episode, int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
   int ep = episode ? episode[i] : 0;
-  rs_fetch_reset_record(p, seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_qpos, st_goal, state + (size_t)i * stride);
+  rs_fetch_reset_record(p, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_qpos, st_goal, state + (size_t)i * stride);
   if (episode) episode[i] = ep + 1;
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
 
-__global__ void uniform_reset_kernel(b200sim_uniform_reset_t p, unsigned long long seed, int env_offset, int N, const unsigned char* __restrict__ mask,
+__global__ void uniform_reset_kernel(b200sim_uniform_reset_t p, unsigned long long seed, const unsigned long long* __restrict__ keys, int env_offset, int N,
+                                     const unsigned char* __restrict__ mask,
                                      const float* __restrict__ rest, int stride, float* __restrict__ state, int* __restrict__ episode, int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
   int ep = episode ? episode[i] : 0;
-  rs_uniform_reset_record(p, seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, state + (size_t)i * stride);
+  rs_uniform_reset_record(p, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, state + (size_t)i * stride);
   if (episode) episode[i] = ep + 1;
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
 
 __global__ void maze_reset_kernel(b200sim_maze_reset_t p, const float* __restrict__ goal_xy, const float* __restrict__ reset_xy, unsigned long long seed,
-                                  int env_offset, int N, const unsigned char* __restrict__ mask, const float* __restrict__ rest, int stride,
+                                  const unsigned long long* __restrict__ keys, int env_offset, int N, const unsigned char* __restrict__ mask, const float* __restrict__ rest, int stride,
                                   int st_qpos, int st_goal, float* __restrict__ state, int* __restrict__ episode, int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
   int ep = episode ? episode[i] : 0;
-  rs_maze_reset_record(p, goal_xy, reset_xy, seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_qpos, st_goal, state + (size_t)i * stride);
+  rs_maze_reset_record(p, goal_xy, reset_xy, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_qpos, st_goal, state + (size_t)i * stride);
   if (episode) episode[i] = ep + 1;
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
@@ -88,21 +91,21 @@ struct GoalUpdateArgs {
   int env_offset;
   const int* episode;
 };
-__global__ void maze_goal_update_kernel(GoalUpdateArgs g, float radius, int N, int stride, int st_qpos, int st_goal, float* __restrict__ state,
+__global__ void maze_goal_update_kernel(GoalUpdateArgs g, const unsigned long long* __restrict__ keys, float radius, int N, int stride, int st_qpos, int st_goal, float* __restrict__ state,
                                         const int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   float* rec = state + (size_t)i * stride;
   const float ach[2] = {rec[st_qpos], rec[st_qpos + 1]};
   float goal[2] = {rec[st_goal], rec[st_goal + 1]};
-  if (rs_maze_goal_update(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
+  if (rs_maze_goal_update(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, keys ? keys[i] : g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
                           (uint32_t)elapsed[i], ach, goal)) {
     rec[st_goal] = goal[0]; rec[st_goal + 1] = goal[1];
   }
 }
 // b200sim_set_goal_redraw (AntMaze-v3): the same thread layout and key; one candidate, and the env's reward in the step's outputs
 // (reward[i * reward_stride]: the separate buffer or the packed column) is written again against the new goal
-__global__ void maze_goal_redraw_kernel(GoalUpdateArgs g, float radius, int dense, int N, int stride, int st_qpos, int st_goal,
+__global__ void maze_goal_redraw_kernel(GoalUpdateArgs g, const unsigned long long* __restrict__ keys, float radius, int dense, int N, int stride, int st_qpos, int st_goal,
                                         float* __restrict__ state, const int* __restrict__ elapsed, float* __restrict__ reward,
                                         int reward_stride) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -110,7 +113,7 @@ __global__ void maze_goal_redraw_kernel(GoalUpdateArgs g, float radius, int dens
   float* rec = state + (size_t)i * stride;
   const float ach[2] = {rec[st_qpos], rec[st_qpos + 1]};
   float goal[2] = {rec[st_goal], rec[st_goal + 1]}, r;
-  if (rs_maze_goal_redraw(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, dense, g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
+  if (rs_maze_goal_redraw(g.goal_xy, g.n_goal, g.scaling, g.noise, radius, dense, keys ? keys[i] : g.seed, (uint32_t)(i + g.env_offset), (uint32_t)g.episode[i],
                           (uint32_t)elapsed[i], ach, goal, &r)) {
     rec[st_goal] = goal[0]; rec[st_goal + 1] = goal[1];
     reward[(size_t)i * reward_stride] = r;
@@ -124,31 +127,34 @@ __global__ void check_state_kernel(int N, int stride, float* __restrict__ state,
   bad[i] = (unsigned char)rs_check_record(state + (size_t)i * stride, stride, rest, keep);
 }
 
-__global__ void hand_pose_kernel(b200sim_hand_reset_t p, const float* __restrict__ parallel, unsigned long long seed, int env_offset, int N,
+__global__ void hand_pose_kernel(b200sim_hand_reset_t p, const float* __restrict__ parallel, unsigned long long seed,
+                                 const unsigned long long* __restrict__ keys, int env_offset, int N,
                                  const unsigned char* __restrict__ mask, const float* __restrict__ rest, int stride, int st_qpos, int st_goal,
                                  int ngoal, float* __restrict__ state, const int* __restrict__ episode, int attempt) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
-  rs_hand_pose_record(p, parallel, seed, (uint32_t)(i + env_offset), (uint32_t)(episode ? episode[i] : 0), (uint32_t)attempt, rest, stride, st_qpos,
+  rs_hand_pose_record(p, parallel, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)(episode ? episode[i] : 0), (uint32_t)attempt, rest, stride, st_qpos,
                       st_goal, ngoal, state + (size_t)i * stride);
 }
-__global__ void hand_goal_kernel(b200sim_hand_reset_t p, const float* __restrict__ parallel, unsigned long long seed, int env_offset, int N,
+__global__ void hand_goal_kernel(b200sim_hand_reset_t p, const float* __restrict__ parallel, unsigned long long seed,
+                                 const unsigned long long* __restrict__ keys, int env_offset, int N,
                                  const unsigned char* __restrict__ mask, int stride, int st_qpos, int st_goal, float* __restrict__ state,
                                  int* __restrict__ episode, int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
   int ep = episode ? episode[i] : 0;
-  rs_hand_goal(p, parallel, seed, (uint32_t)(i + env_offset), (uint32_t)ep, st_qpos, st_goal, state + (size_t)i * stride);
+  rs_hand_goal(p, parallel, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)ep, st_qpos, st_goal, state + (size_t)i * stride);
   if (episode) episode[i] = ep + 1;
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
 
-__global__ void reach_reset_kernel(b200sim_reach_reset_t p, unsigned long long seed, int env_offset, int N, const unsigned char* __restrict__ mask,
+__global__ void reach_reset_kernel(b200sim_reach_reset_t p, unsigned long long seed, const unsigned long long* __restrict__ keys, int env_offset, int N,
+                                   const unsigned char* __restrict__ mask,
                                    const float* __restrict__ rest, int stride, int st_goal, float* __restrict__ state, int* __restrict__ episode, int* __restrict__ elapsed) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N || (mask && !mask[i])) return;
   int ep = episode ? episode[i] : 0;
-  rs_reach_reset_record(p, seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_goal, state + (size_t)i * stride);
+  rs_reach_reset_record(p, keys ? keys[i] : seed, (uint32_t)(i + env_offset), (uint32_t)ep, rest, stride, st_goal, state + (size_t)i * stride);
   if (episode) episode[i] = ep + 1;
   if (elapsed) elapsed[i] = 0;   // a reset env starts a new episode of the TimeLimit
 }
@@ -183,7 +189,8 @@ struct b200sim {
   unsigned long long* overflow_count = nullptr;  // env-steps that hit a capacity limit (device counter)
   int max_steps = 0, term_on_success = 0;        // b200sim_set_time_limit
   int packed = 0, packed_w = 0;                  // b200sim_set_packed
-  ObsNoiseArgs noise = {nullptr, nullptr, 0, 0};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
+  ObsNoiseArgs noise = {nullptr, nullptr, 0, 0, nullptr};  // b200sim_set_obs_noise (kitchen units): scale NULL = noise-free observations
+  const unsigned long long* keys = nullptr;     // b200sim_set_env_keys: per-env Philox keys of every draw (device, [N]; NULL = the seeds)
   GoalUpdateArgs goal_update = {nullptr, 0, 0.f, 0.f, 0, 0, nullptr};   // b200sim_set_goal_update / b200sim_set_goal_redraw (maze tasks)
   int goal_redraw = 0;                                                  // 1: the slot above is b200sim_set_goal_redraw's
   // b200sim_set_ant_info (ant build): Ant-v5's defaults, no info rows until set
@@ -431,7 +438,9 @@ static int launch(b200sim* h, int mode, int nraw, const float* actions, const un
   io.terminated = terminated; io.truncated = truncated; io.info = info;
   io.elapsed = h->elapsed; io.max_steps = h->max_steps; io.term_on_success = h->term_on_success; io.overflow_count = h->overflow_count;
   ON_DEVICE(h);
-  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io, h->noise, h->ant))
+  ObsNoiseArgs noise = h->noise;
+  noise.keys = h->keys;
+  if (!h->unit->launch(h->wpb, h->nvp, h->blocks, h->smem_bytes, (cudaStream_t)stream, h->model_dev, h->task, mode, nraw, h->N, io, noise, h->ant))
     return fail(h, "no kernel variant for this (envs per block, nv) pair: nothing was launched", -8);
   h->launches++;
   CUDA_OK(cudaGetLastError());
@@ -448,11 +457,11 @@ int b200sim_step(b200sim_t* h, const float* actions, float* obs, float* achieved
   const FetchTask& t = h->task;
   if (h->goal_redraw) {
     float* rew = h->packed ? obs + t.nobs + 2 * t.ngoal : reward;   // the reward column of the packed row (launch) or the buffer
-    maze_goal_redraw_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, t.success_radius, t.reward_dense, h->N,
+    maze_goal_redraw_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->keys, t.success_radius, t.reward_dense, h->N,
                                                                                  t.st_stride, t.st_qpos, t.st_goal, h->state, h->elapsed, rew,
                                                                                  h->packed ? h->packed_w : 1);
   } else {
-    maze_goal_update_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->task.success_radius, h->N, h->task.st_stride,
+    maze_goal_update_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->goal_update, h->keys, h->task.success_radius, h->N, h->task.st_stride,
                                                                                  h->task.st_qpos, h->task.st_goal, h->state, h->elapsed);
   }
   h->launches++;
@@ -493,7 +502,11 @@ int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long s
     return fail(h, "b200sim_set_obs_noise: observation noise exists in the kitchen kernel builds only", -6);
   if (scale && !episode) return fail(h, "b200sim_set_obs_noise: episode is NULL", -1);
   if (env_offset < 0) return fail(h, "b200sim_set_obs_noise: negative env_offset", -1);
-  h->noise = {scale, scale ? episode : nullptr, seed, env_offset};
+  h->noise = {scale, scale ? episode : nullptr, seed, env_offset, nullptr};
+  return 0;
+}
+int b200sim_set_env_keys(b200sim_t* h, const unsigned long long* keys) {
+  h->keys = keys;
   return 0;
 }
 int b200sim_refresh(b200sim_t* h, const unsigned char* mask, float* obs, float* achieved, float* desired, float* reward,
@@ -508,7 +521,7 @@ int b200sim_reset(b200sim_t* h, const unsigned char* mask, const float* rest_rec
   if (params->has_object && (params->obj_qadr < 0 || params->obj_qadr + 2 > h->task.st_qvel - h->task.st_qpos)) return fail(h, "b200sim_reset: obj_qadr outside qpos", -1);
   {
     ON_DEVICE(h);
-    fetch_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, env_offset, h->N, mask, rest_record, h->task.st_stride,
+    fetch_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, h->keys, env_offset, h->N, mask, rest_record, h->task.st_stride,
                                                                             h->task.st_qpos, h->task.st_goal, h->state, episode, h->elapsed);
     h->launches++;
     CUDA_OK(cudaGetLastError());
@@ -525,7 +538,7 @@ int b200sim_reset_uniform(b200sim_t* h, const unsigned char* mask, const float* 
   if (params->quat_slot < -1 || params->quat_slot + 4 > h->task.st_stride) return fail(h, "b200sim_reset_uniform: quat_slot outside the state record", -1);
   {
     ON_DEVICE(h);
-    uniform_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, env_offset, h->N, mask, rest_record, h->task.st_stride,
+    uniform_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, h->keys, env_offset, h->N, mask, rest_record, h->task.st_stride,
                                                                               h->state, episode, h->elapsed);
     h->launches++;
     CUDA_OK(cudaGetLastError());
@@ -540,7 +553,7 @@ int b200sim_reset_maze(b200sim_t* h, const unsigned char* mask, const float* res
   if (params->n_goal < 1 || params->n_reset < 1) return fail(h, "b200sim_reset_maze: empty cell table", -1);
   {
     ON_DEVICE(h);
-    maze_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, goal_xy, reset_xy, seed, env_offset, h->N, mask, rest_record,
+    maze_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, goal_xy, reset_xy, seed, h->keys, env_offset, h->N, mask, rest_record,
                                                                            h->task.st_stride, h->task.st_qpos, h->task.st_goal, h->state, episode, h->elapsed);
     h->launches++;
     CUDA_OK(cudaGetLastError());
@@ -560,7 +573,7 @@ int b200sim_reset_hand_pose(b200sim_t* h, const unsigned char* mask, const float
   if (int rc = hand_reset_args(h, params, parallel_quats)) return rc;
   if (!rest_record) return fail(h, "b200sim_reset_hand_pose: rest_record is NULL", -1);
   ON_DEVICE(h);
-  hand_pose_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, parallel_quats, seed, env_offset, h->N, mask, rest_record,
+  hand_pose_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, parallel_quats, seed, h->keys, env_offset, h->N, mask, rest_record,
                                                                         h->task.st_stride, h->task.st_qpos, h->task.st_goal, h->task.ngoal, h->state,
                                                                         episode, attempt);
   h->launches++;
@@ -573,7 +586,7 @@ int b200sim_reset_hand_goal(b200sim_t* h, const unsigned char* mask, const b200s
   if (int rc = hand_reset_args(h, params, parallel_quats)) return rc;
   {
     ON_DEVICE(h);
-    hand_goal_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, parallel_quats, seed, env_offset, h->N, mask, h->task.st_stride,
+    hand_goal_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, parallel_quats, seed, h->keys, env_offset, h->N, mask, h->task.st_stride,
                                                                           h->task.st_qpos, h->task.st_goal, h->state, episode, h->elapsed);
     h->launches++;
     CUDA_OK(cudaGetLastError());
@@ -587,7 +600,7 @@ int b200sim_reset_reach(b200sim_t* h, const unsigned char* mask, const float* re
   if (!rest_record || !params) return fail(h, "b200sim_reset_reach: NULL argument", -1);
   {
     ON_DEVICE(h);
-    reach_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, env_offset, h->N, mask, rest_record, h->task.st_stride,
+    reach_reset_kernel<<<(h->N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*params, seed, h->keys, env_offset, h->N, mask, rest_record, h->task.st_stride,
                                                                             h->task.st_goal, h->state, episode, h->elapsed);
     h->launches++;
     CUDA_OK(cudaGetLastError());

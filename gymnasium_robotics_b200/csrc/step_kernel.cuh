@@ -30,10 +30,10 @@ struct StepIO {
 };
 
 // The observation noise of a handle (b200sim_set_obs_noise): one scale per observation entry (NULL = no noise), the per-env
-// episode counters, the key and the global index of env 0.  A kernel parameter of the kitchen builds only: the other builds' kernels
-// take exactly the parameters they took before it existed.
+// episode counters, the key, the global index of env 0 and the per-env keys that replace `seed` (b200sim_set_env_keys; NULL = none).
+// A kernel parameter of the kitchen builds only: the other builds' kernels take exactly the parameters they took before it existed.
 struct ObsNoiseArgs {
-  const float* scale; const int* episode; unsigned long long seed; int env_offset;
+  const float* scale; const int* episode; unsigned long long seed; int env_offset; const unsigned long long* keys;
 };
 #ifdef B200_KITCHEN
 #define B200_KITCHEN_PARAM , ObsNoiseArgs noise_args
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(WPB * 32) fetch_kernel(const uint32_t* __restr
   // the noise of the observation this launch returns: the episode that observation belongs to and the step count after the launch
   // (a step increments `elapsed` below; a refresh -- after a reset, after set_state -- leaves it)
   const bool noisy = active && noise_args.scale;
-  const ObsNoiseKey noise_key = {noise_args.scale, noise_args.seed, (uint32_t)(noise_args.env_offset + env), noisy ? (uint32_t)noise_args.episode[e] : 0u,
+  const ObsNoiseKey noise_key = {noise_args.scale, noisy && noise_args.keys ? noise_args.keys[e] : noise_args.seed, (uint32_t)(noise_args.env_offset + env), noisy ? (uint32_t)noise_args.episode[e] : 0u,
                                  noisy ? (uint32_t)(io.elapsed[e] + (mode == MODE_STEP ? 1 : 0)) : 0u};
   fetch_env_step<NVP, (WPB >= 28)>(c, task, active, mode, nraw, io.state + e * task.st_stride, act, io.obs + e * io.obs_stride, io.achieved + e * io.goal_stride,
                       io.desired + e * io.goal_stride, io.reward + e * io.scalar_stride, success, &iters, noisy ? &noise_key : nullptr);

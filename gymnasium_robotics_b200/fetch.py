@@ -204,6 +204,14 @@ class CudaBackend:
         self._check(self.L.b200sim_set_obs_noise(self.h, scale.data_ptr() if scale is not None else None, int(seed) & 0xFFFFFFFFFFFFFFFF,
                                                  int(env_offset), episode.data_ptr() if scale is not None else None))
 
+    def set_env_keys(self, keys):
+        """b200sim_set_env_keys: every later draw of env i (resets, goal update / redraw, observation noise) is keyed by keys[i]
+        (int64 [N] on the device, read as unsigned) in place of the seed; None turns the table off.  The handle keeps the pointer:
+        the tensor must outlive its launches."""
+        if keys is not None:
+            assert keys.is_cuda and keys.dtype == torch.int64 and keys.is_contiguous() and keys.numel() == self.num_envs
+        self._check(self.L.b200sim_set_env_keys(self.h, keys.data_ptr() if keys is not None else None))
+
     def set_goal_update(self, goal_xy, scaling, noise, seed, env_offset, episode, fn="b200sim_set_goal_update"):
         """b200sim_set_goal_update (maze tasks): every later step redraws the goal of the envs that succeeded, per (seed, env,
         episode, step); goal_xy None turns the update off.  The handle keeps both pointers: the tensors must outlive its steps."""
@@ -402,7 +410,6 @@ class FetchVectorEnv(VectorEnv):
         if self.rng_mode == "device":
             if self._dev_reset is None:
                 self._dev_reset = self._device_reset_params()
-                self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
             p, rest = self._dev_reset
             every = self._reset_all
             self.backend.reset_draw(None if every else mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)

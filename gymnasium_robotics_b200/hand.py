@@ -250,7 +250,6 @@ class HandVectorEnv(VectorEnv):
             for k in range(3):
                 p.pos_lo[k], p.pos_hi[k] = float(TARGET_POSITION_RANGE[k, 0]), float(TARGET_POSITION_RANGE[k, 1])
             self._dev_reset = (p, self._rest, self._parallel.contiguous())
-            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         p, rest, par = self._dev_reset
         st = self.backend.state
         pending = mask.clone()
@@ -429,7 +428,6 @@ class HandReachVectorEnv(VectorEnv):
             for k in range(15):
                 p.initial_goal[k] = float(init[k])
             self._dev_reset = (p, self._rest)
-            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         p, rest = self._dev_reset
         self.backend.reset_reach(mask.to(torch.uint8), rest, p, self._dev_seed, self.env_offset, self._episode, out)
         self._elapsed.masked_fill_(mask, 0)

@@ -23,7 +23,7 @@ from ._lib import FetchTaskC
 from .fetch import KITCHEN_REF_POINT, CudaBackend  # noqa: F401  (KITCHEN_REF_POINT: re-exported)
 from .models import load_franka_config, load_model
 from .spaces import Box
-from .vector import VectorEnv
+from .vector import VectorEnv, _int64
 
 FRAME_SKIP = 40
 # kitchen_env.py:27-45
@@ -62,7 +62,7 @@ class KitchenVectorEnv(VectorEnv):
     the host and have no `set_state`.  rng_mode="device" draws it in the step kernel (b200sim_set_obs_noise) as a function of
     (seed, global env index, episode, step), so a run does not depend on batch shape or sharding, and `get_state` / `set_state`
     checkpoint the env: the record's goal slot, which the kitchen task does not use, carries what the state record lacks --
-    word 0 the episode counter, words 1-2 the seed (int32 bits), then `tasks_to_complete` and `episode_task_completions` (0 / 1)."""
+    word 0 the episode counter, words 1-2 the env's Philox key (int32 bits, low word first), then `tasks_to_complete` and `episode_task_completions` (0 / 1)."""
 
     metadata = {"render_modes": [], "render_fps": 12, "autoreset_mode": "next_step"}
     AUTO_RECOVER = False
@@ -188,7 +188,6 @@ class KitchenVectorEnv(VectorEnv):
             p = UniformResetC()
             p.n, p.quat_slot = 0, -1   # reset_model draws nothing but the observation noise
             self._dev_reset = p
-            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
         self.backend.set_obs_noise(self._noise_scale, self._dev_seed, self.env_offset, self._episode)
         return self._dev_reset
 
@@ -275,9 +274,8 @@ class KitchenVectorEnv(VectorEnv):
             self._device_noise()
             g, k = self.backend.layout["goal"], len(self.tasks)
             state[:, g].view(torch.int32).copy_(self._episode)
-            seed = self._dev_seed & 0xFFFFFFFFFFFFFFFF
-            words = torch.tensor([seed & 0xFFFFFFFF, seed >> 32], dtype=torch.int64).to(torch.int32)   # two's-complement wrap
-            state[:, g + 1:g + 3].view(torch.int32).copy_(words.to(self.device).expand(self.num_envs, 2))
+            keys = self._keys if self._keys is not None else torch.full((self.num_envs,), _int64(self._dev_seed), dtype=torch.int64, device=self.device)
+            state[:, g + 1:g + 3].view(torch.int32).copy_(keys.view(torch.int32).view(self.num_envs, 2))   # each env's key, low word first
             state[:, g + 3:g + 3 + k] = self._todo.to(torch.float32)
             state[:, g + 3 + k:g + 3 + 2 * k] = self._episode_done.to(torch.float32)
         return state, elapsed
@@ -291,8 +289,10 @@ class KitchenVectorEnv(VectorEnv):
         state = torch.as_tensor(state).to(self.device, torch.float32)
         g, k = self.backend.layout["goal"], len(self.tasks)
         words = state[:, g:g + 3].contiguous().view(torch.int32)
-        lo, hi = (int(w) & 0xFFFFFFFF for w in words[0, 1:3].tolist())
-        self._dev_seed = lo | (hi << 32)
+        keys = words[:, 1:3].contiguous().view(torch.int64).view(self.num_envs)
+        self._dev_seed = int(keys[0]) & 0xFFFFFFFFFFFFFFFF   # the noise seed of a backend without per-env keys
+        if self._keys is not None:
+            self._keys.copy_(keys)
         self._device_noise()
         self._episode.copy_(words[:, 0])
         self._todo = state[:, g + 3:g + 3 + k] != 0

@@ -329,7 +329,7 @@ class MazeVectorEnv(VectorEnv):
         self._goal_loc = torch.as_tensor(self.cells.goal_locations, dtype=torch.float32, device=self.device)
         self._reset_loc = torch.as_tensor(self.cells.reset_locations, dtype=torch.float32, device=self.device)
         # update_goal (maze_v4.py:400-418) acts only in a continuing task with reset_target and more than one goal location; in
-        # rng_mode="device" the step launch does it (b200sim_set_goal_update), keyed by the seed the library was last given
+        # rng_mode="device" the step launch does it (b200sim_set_goal_update), keyed by each env's Philox key (vector.py)
         self._goal_update_on = continuing_task and reset_target and len(self.cells.goal_locations) > 1
         # AntMaze-v3's redraw (maze.py:283-302) acts in a continuing task with more than one goal location; in rng_mode="device" the
         # step launch does it (b200sim_set_goal_redraw), rewriting the reward too
@@ -395,8 +395,8 @@ class MazeVectorEnv(VectorEnv):
             p.n_goal, p.n_reset, p.scaling, p.noise = len(self._goal_loc), len(self._reset_loc), float(self.scaling), float(NOISE)
             p.separation = self.separation if self._v3 else 0.0   # 0: the library's half cell, bit for bit the v4 draw
             self._dev_reset = (p, self._rest, self._goal_loc.contiguous(), self._reset_loc.contiguous())
-            self._episode = torch.zeros(self.num_envs, dtype=torch.int32, device=self.device)
-        if (self._goal_update_on or self._goal_redraw_on) and self._goal_update_seed != self._dev_seed:   # first reset, or a new key
+        # first reset, or a new seed: the slot's seed keys the draws of a backend without per-env keys (vector.py)
+        if (self._goal_update_on or self._goal_redraw_on) and self._goal_update_seed != self._dev_seed:
             setter = self.backend.set_goal_redraw if self._goal_redraw_on else self.backend.set_goal_update
             setter(self._dev_reset[2], self.scaling, NOISE, self._dev_seed, self.env_offset, self._episode)
             self._goal_update_seed = self._dev_seed

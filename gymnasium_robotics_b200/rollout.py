@@ -11,7 +11,7 @@
 The recorder understands the three autoreset modes of the vector envs: in `next_step` mode the call after an episode end
 is the reset call (its action is ignored and its reward is zero), so that row is dropped from the data and its observation
 opens the next episode; in `same_step` mode the last observation of an episode is `info["final_obs"]`; in `disabled` mode
-the caller resets and calls `mark_reset()`.
+the caller resets and calls `mark_reset()`, with the reset mask when only some envs were reset.
 """
 from __future__ import annotations
 
@@ -118,9 +118,23 @@ class RolloutRecorder:
         self.t = 0
         return obs, info
 
-    def mark_reset(self, obs):
-        """`disabled` autoreset: the caller reset (some of) the envs; `obs` is the full batch of current observations."""
-        self._cur = {k: v.clone() for k, v in _flatten_obs(obs).items()}
+    def mark_reset(self, obs, mask=None):
+        """`disabled` autoreset: the caller reset (some of) the envs; `obs` is the full batch of current observations (what
+        `reset(options={"reset_mask": mask})` returns).  Without `mask` every env continues from `obs`.  With `mask` (bool, [num_envs],
+        numpy or torch) only the masked envs' open episodes end here and their rows of `obs` open their next episode; the others
+        go on as if nothing happened.  An episode cut this way before it terminated or was truncated gets `truncations=True` on its
+        last row: from the agent's side it was cut short."""
+        flat = _flatten_obs(obs)
+        if mask is None:
+            self._cur = {k: v.clone() for k, v in flat.items()}
+            return
+        dev = next(iter(flat.values())).device
+        mask = torch.as_tensor(mask).to(dev, torch.bool)
+        if self._buf is not None and self.t > 0:
+            b, t = self._buf, self.t - 1
+            b["truncations"][t] |= mask & ~b["terminations"][t]
+        for k, v in flat.items():
+            self._cur[k] = torch.where(mask.reshape((-1,) + (1,) * (v.dim() - 1)), v, self._cur[k])
 
     def _alloc(self, act, flat):
         T, dev = self.capacity, act.device

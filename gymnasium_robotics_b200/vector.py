@@ -26,6 +26,12 @@ def _clone(x):
     return {k: _clone(v) for k, v in x.items()} if isinstance(x, dict) else x.clone()
 
 
+def _int64(seed):
+    """A seed as the signed 64-bit word the library reads back as unsigned."""
+    s = int(seed) & 0xFFFFFFFFFFFFFFFF
+    return s - (1 << 64) if s >= 1 << 63 else s
+
+
 class VectorEnv(CtorPickle):
     """Observations, rewards and flags are torch tensors on `device` with a leading `num_envs` axis."""
 
@@ -82,7 +88,15 @@ class VectorEnv(CtorPickle):
         # autoreset state: `_elapsed_ub` is a host-side upper bound of max(_elapsed); `_in_phase`: every env was reset together and
         # none can terminate, so the bound IS every env's step count and the TimeLimit is known without reading the device
         self._elapsed_ub, self._pending_reset, self._in_phase, self._reset_all = 0, False, False, False
-        self._episode = self._dev_reset = self._recovery = None   # built by the first device reset / recovery
+        self._episode = self._keys = self._dev_reset = self._recovery = None   # built below / by the first device reset / recovery
+        if self.rng_mode == "device":
+            # per-env episode counters and Philox keys of the library's draws (b200sim_set_env_keys): a full reset with a seed gives every
+            # env that key, a partial one gives it to the envs it resets and leaves the others' streams alone.  A backend without
+            # the hook draws every env with the batch seed and refuses only a partial reset with a seed
+            self._episode = torch.zeros(n, dtype=torch.int32, device=dev)
+            if getattr(self.backend, "set_env_keys", None) is not None:
+                self._keys = torch.full((n,), _int64(self._dev_seed), dtype=torch.int64, device=dev)
+                self.backend.set_env_keys(self._keys)
         self._last = None
         self.closed = False
 
@@ -116,21 +130,87 @@ class VectorEnv(CtorPickle):
     def _reset_info(self, out):
         return {}
 
+    def _seeds(self, seed):
+        return [seed + i for i in range(self.num_envs)] if isinstance(seed, (int, np.integer)) else list(seed)
+
     def reset(self, *, seed=None, options=None):
+        """Gymnasium's vector reset.  `options={"reset_mask": mask}` resets only the envs in `mask` (a numpy bool array of shape
+        (num_envs,), Gymnasium's form, with at least one True; or a torch.bool tensor, the GPU-native form, which is not read, so an
+        all-False one is a no-op); the other options go to the family's reset.  The whole batch comes back: the masked rows hold
+        their new episode's first observation, the others their current one.  A reset of mask M with `seed=x` leaves each env of M
+        as a full `reset(seed=x)` would (record, observation, step counter and RNG stream) and every other env as it was: in
+        rng_mode="numpy" env i of M gets the generator of seed x + i (or x[i]); in "device" it gets the key x (or x[0]) and its
+        episode counter restarts, so it replays its episode of a full reset bit for bit, later goal updates and observation noise
+        included; in "torch" x reseeds the one device generator and the masked envs draw from it, which promises equal
+        distributions only.  With seed=None the masked envs continue their own streams."""
+        if options and "reset_mask" in options:
+            options = dict(options)
+            mask, every = self._reset_mask(options.pop("reset_mask"))
+            return self._partial_reset(mask, every, seed, options or None)
         if seed is not None:
-            seeds = [seed + i for i in range(self.num_envs)] if isinstance(seed, (int, np.integer)) else list(seed)
+            seeds = self._seeds(seed)
             if self._np_rngs is not None:
                 self._np_rngs = self._new_np_rngs(seeds)
             self._gen.manual_seed(int(seeds[0]))
             self._dev_seed = int(seeds[0])   # rng_mode="device": one key for the batch; env index and episode counter select the stream
             if self._episode is not None:
                 self._episode.zero_()
+            if self._keys is not None:
+                self._keys.fill_(_int64(self._dev_seed))
         out = self.backend.new_outputs()
         self._reset(torch.ones(self.num_envs, dtype=torch.bool, device=self.device), out, True, options)
         self._needs_reset.zero_()
         self._elapsed_ub, self._pending_reset, self._in_phase = 0, False, not self._can_terminate
         self._last = out
         return self._obs_dict(out), self._reset_info(out)
+
+    def _reset_mask(self, mask):
+        """The mask on the device, and whether it holds every env (None for a torch mask: finding out would read the device)."""
+        shape = (self.num_envs,)
+        if isinstance(mask, np.ndarray):
+            if mask.dtype != np.bool_ or mask.shape != shape:
+                raise ValueError(f"reset_mask must be a bool array of shape {shape}, got {mask.dtype} {mask.shape}")
+            if not mask.any():
+                raise ValueError("reset_mask has no True entry: no env would be reset")
+            return torch.from_numpy(mask).to(self.device), bool(mask.all())
+        if torch.is_tensor(mask):
+            if mask.dtype != torch.bool or tuple(mask.shape) != shape:
+                raise ValueError(f"reset_mask must be a torch.bool tensor of shape {shape}, got {mask.dtype} {tuple(mask.shape)}")
+            return mask.to(self.device), None
+        raise ValueError(f"reset_mask must be a numpy bool array or a torch.bool tensor, got {type(mask).__name__}")
+
+    def _partial_reset(self, mask, every, seed, options):
+        if seed is not None and self.rng_mode == "device" and self._keys is None:
+            raise NotImplementedError(f"a partial reset with a seed in rng_mode='device' needs per-env keys (set_env_keys, "
+                                      f"b200sim_set_env_keys); {type(self.backend).__name__} has none")
+        if seed is not None:
+            seeds = self._seeds(seed)
+            if self._np_rngs is not None:   # the host streams need the mask on the host
+                for i in torch.nonzero(mask.cpu(), as_tuple=False).flatten().tolist():
+                    self._np_rngs[i] = self._new_np_rngs([seeds[i]])[0]
+            self._gen.manual_seed(int(seeds[0]))
+            if self._keys is not None:
+                self._keys.masked_fill_(mask, _int64(seeds[0]))
+                self._episode.masked_fill_(mask, 0)
+        out = self.backend.new_outputs()
+        if self._last is not None:   # the rows outside the mask keep their current observation
+            out["packed"].copy_(self._last["packed"])
+            out["packed"].masked_fill_(mask[:, None], 0.0)
+            out["flags"].copy_(self._last["flags"])
+            out["flags"].masked_fill_(mask[None, :], 0)
+        self._reset(mask, out, False, options)
+        self._needs_reset = self._needs_reset & ~mask   # a pending NEXT_STEP autoreset of a masked env is cancelled
+        # the step bound stays valid (reset envs count from 0); the envs are in phase again only when every one was reset
+        if every:
+            self._elapsed_ub, self._pending_reset, self._in_phase = 0, False, not self._can_terminate
+        else:
+            self._in_phase = False
+        self._last = out
+        info = self._reset_info(out)
+        for k in info:
+            if k.startswith("_"):
+                info[k] = mask
+        return self._obs_dict(out), info
 
     # step hooks: the defaults serve the families whose step results are the packed row's columns
     def _kernel_input(self, actions):

@@ -159,6 +159,14 @@ int b200sim_reset_uniform(b200sim_t* h, const unsigned char* mask, const float* 
  * that b200sim_reset_uniform increments) are read by every later launch and must outlive them.  scale NULL: noise off.  The
  * `achieved` columns (qpos) stay noise-free.  A reset is b200sim_reset_uniform with n = 0 draws. */
 int b200sim_set_obs_noise(b200sim_t* h, const float* scale, unsigned long long seed, int env_offset, const int* episode);
+/* Per-env Philox keys.  keys: DEVICE [N] unsigned 64-bit words, read by every later launch and must outlive them; NULL turns the
+ * table off.  While it is set, every Philox draw of the handle keys env i with keys[i] in place of the `seed` argument of the reset
+ * entry points or the seed stored by b200sim_set_obs_noise / b200sim_set_goal_update / b200sim_set_goal_redraw: the reset draws, the
+ * goal update and redraw after b200sim_step, and the observation noise of step and refresh launches.  The counters are unchanged
+ * (env index + env_offset, episode, step, tag).  A table whose entries all equal the seed gives the same draws as no table; a
+ * caller that changes one env's key (and zeroes its episode counter) restarts that env's streams alone, which is what a reset of
+ * some envs with a new seed needs.  Handles that never set a table draw as before. */
+int b200sim_set_env_keys(b200sim_t* h, const unsigned long long* keys);
 /* Maze family (AntMaze / PointMaze; reference: envs/maze/maze_v4.py:256-297, 299-373): goal cell + noise, reset cell farther than
  * half a cell from the goal + noise.  goal_xy / reset_xy: DEVICE tables [n_goal, 2] / [n_reset, 2] of cell centres
  * (MazeEnv.maze.unique_goal_locations / unique_reset_locations, or all free cells when the map marks none, maze_v4.py:212-228). */
