@@ -31,6 +31,10 @@
 // block-wide alignment points: keep the warps of a block inside the same code window (instruction-cache locality)
 #define ALIGN() __syncthreads()
 #define ALIGN_OR(p) __syncthreads_or(p)
+// loops over run-time counts stay rolled (LANES and the walks of the solver stages): nvcc unrolls them by four with remainder code,
+// and a lane loop over at most 32 items runs once per lane, so the copies only add to the code every warp streams (DESIGN.md 3,
+// "Footprint of the Newton iteration"); the order of the floating-point operations is the same either way
+#define ROLLED _Pragma("unroll 1")
 #elif defined(B200_HOST_WARP)
 #define HD static inline
 #define HDN static
@@ -53,6 +57,9 @@ static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
 #define ALIGN() do { } while (0)
 #define ALIGN_OR(p) (p)
 static inline float rsqrtf(float x) { return 1.0f / sqrtf(x); }
+#endif
+#ifndef ROLLED
+#define ROLLED
 #endif
 
 #define B200_MINVAL 1e-15f
@@ -122,7 +129,7 @@ HD Ctx stage_ctx(const Ctx& c) {
 #define GF(name) ((const float*)(c.mg + c.h->o_##name))
 #define SF(name) (c.s + c.h->s_##name)
 #define SI(name) ((int*)(c.s + c.h->s_##name))
-#define LANES(i, n) for (int i = c.lane; i < (n); i += WARP_W)
+#define LANES(i, n) ROLLED for (int i = c.lane; i < (n); i += WARP_W)
 
 // ---------------------------------------------------------------------------------------------------------------
 // warp helpers
@@ -1804,7 +1811,7 @@ HD void pass_F(const Ctx c, float* out) {
     int g = idx / 6, a = idx - 6 * g;
     float* gr = SF(group) + g * GRP_WORDS;
     float acc = 0;
-    for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
+    ROLLED for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
       const float* cr = SF(con) + i * CON_WORDS;
       int dim = con_dim(cr);
       const float* F = cr + C_JV;
@@ -1815,7 +1822,7 @@ HD void pass_F(const Ctx c, float* out) {
       if (dim > 4 && a < 3) acc += F[4] * cr[C_W + 6 + 3 + a] + F[5] * cr[C_W + 12 + 3 + a];
 #endif
     }
-    for (int i = 0; i < nweld; i++) {
+    ROLLED for (int i = 0; i < nweld; i++) {
       const float* wr = SF(weld) + i * WELD_WORDS;
       if (((const int*)wr)[W_GRP] != g) continue;
       for (int k = 0; k < 6; k++) acc -= wr[W_D + k] * wr[W_JAR + k] * wr[W_W + 6 * k + a];
@@ -1826,13 +1833,13 @@ HD void pass_F(const Ctx c, float* out) {
   LANES(j, h->nv) {
     float q = 0;
     const float* cd = SF(cdof) + 6 * j;
-    for (int g = 0; g < ngrp; g++) {
+    ROLLED for (int g = 0; g < ngrp; g++) {
       const float* gr = SF(group) + g * GRP_WORDS;
       if (!DBIT(grp_mask(gr), j)) continue;
       float d = dot6(cd, gr + G_V);
       q += DBIT(grp_sign(gr), j) ? d : -d;
     }
-    for (int i = 0; i < ndr; i++) {
+    ROLLED for (int i = 0; i < ndr; i++) {
       const float* dr = SF(dofrow) + i * DR_WORDS;
       const int* di = (const int*)dr;
       float x = dr[DR_JAR];
@@ -1888,11 +1895,11 @@ STAGE void build_H(const Ctx c) {
     LANES(e, 21) {
       int r = 0; while ((r + 1) * (r + 2) / 2 <= e) r++;
       const int s = e - r * (r + 1) / 2;
-      for (int g = g0; g < g1; g++) {
+      ROLLED for (int g = g0; g < g1; g++) {
         float* K = Kc + 21 * (g - g0);
         const float* gr = SF(group) + g * GRP_WORDS;
         float acc = 0;
-        for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
+        ROLLED for (int i = grp_start(gr), i1 = i + grp_count(gr); i < i1; i++) {
           const float* cr = SF(con) + i * CON_WORDS;
           const int dim = con_dim(cr);
           const uint32_t act = con_act(cr);
@@ -1917,7 +1924,7 @@ STAGE void build_H(const Ctx c) {
           }
           acc += D * Wnn * wnr * wns;
         }
-        for (int i = 0; i < nweld; i++) {
+        ROLLED for (int i = 0; i < nweld; i++) {
           const float* wr = SF(weld) + i * WELD_WORDS;
           if (((const int*)wr)[W_GRP] != g) continue;
           for (int k = 0; k < 6; k++) acc += wr[W_D + k] * wr[W_W + 6 * k + r] * wr[W_W + 6 * k + s];
@@ -1931,7 +1938,7 @@ STAGE void build_H(const Ctx c) {
     LANES(i, nv) {
       const float* cd = SF(cdof) + 6 * i;
       const int row = i * (i + 1) / 2;
-      for (int g = g0; g < g1; g++) {
+      ROLLED for (int g = g0; g < g1; g++) {
         const float* gr = SF(group) + g * GRP_WORDS;
         const dmask_t S = grp_mask(gr), mb = grp_sign(gr);
         if (!DBIT(S, i)) continue;
@@ -1988,7 +1995,7 @@ STAGE void build_H(const Ctx c) {
     }
   } else if (c.lane == 0) {
     // few limit rows (arm / legged models): one lane walks them
-    for (int i = 0; i < ndr; i++) {
+    ROLLED for (int i = 0; i < ndr; i++) {
       const float* dr = SF(dofrow) + i * DR_WORDS;
       const int* di = (const int*)dr;
       if (!(dr[DR_JAR] < 0)) continue;
@@ -2261,36 +2268,40 @@ HD LsStep linesearch(const Ctx c, float g1, float g2, float gtol, int maxit) {
     const int e = c.lane + WARP_W * j;
     float x0 = 0.f, v = 0.f, D = 0.f;
     if (j > 0) { q += qs; r += rs; if (r >= epc) { r -= epc; q++; } }
-    if (WARP_W * j < nedge) {   // warp-uniform: slots past the last edge stay empty
-      if (e < nce) {   // contact q, pyramid edge r = base row 1 + r / 2, + for even r
-        const float* cr = SF(con) + q * CON_WORDS;
-        const int k = r, dim = con_dim(cr);
-        const float un = cr[C_U], vn = cr[C_JV];
-        if (dim == 1) {
-          if (k == 0) { x0 = un; v = vn; D = cr[C_D]; }
-        } else if (k < 2 * (dim - 1)) {
-          const int b = 1 + (k >> 1);
-          const float mu = con_mu(cr, b), su = (k & 1) ? -cr[C_U + b] : cr[C_U + b], sv = (k & 1) ? -cr[C_JV + b] : cr[C_JV + b];
-          x0 = pyramid_edge(un, mu, su); v = pyramid_edge(vn, mu, sv);
-          D = cr[C_D];
+    // slots past the last edge stay empty (the first test is warp-uniform).  One row address and one set of loads per slot,
+    // whatever the row is (contact q, weld row or dof row): the slots are unrolled, so three branches of loads each cost
+    // instructions in every Newton move
+    if (WARP_W * j < nedge && e < nedge) {
+      const bool isc = e < nce, isw = !isc && e < nwe;
+      const int i = e - (isw ? nce : nwe), o = isw ? i % 6 : 0;
+      const float* row = isc ? SF(con) + q * CON_WORDS : isw ? SF(weld) + (i / 6) * WELD_WORDS : SF(dofrow) + i * DR_WORDS;
+      x0 = row[(isc ? C_U : isw ? W_JAR : DR_JAR) + o];
+      v = row[(isc ? C_JV : isw ? W_JV : DR_JV) + o];
+      D = row[(isc ? C_D : isw ? W_D : DR_D) + o];
+      if (isw) D = -D;
+      if (isc) {   // pyramid edge r = base row 1 + r / 2, + for even r; a frictionless contact has the one edge r = 0
+        const int dim = con_dim(row);
+        if (dim > 1 && r < 2 * (dim - 1)) {
+          const int b = 1 + (r >> 1);
+          const float mu = con_mu(row, b), su = (r & 1) ? -row[C_U + b] : row[C_U + b], sv = (r & 1) ? -row[C_JV + b] : row[C_JV + b];
+          x0 = pyramid_edge(x0, mu, su); v = pyramid_edge(v, mu, sv);
+        } else if (dim > 1 || r != 0) {
+          x0 = 0.f; v = 0.f; D = 0.f;
         }
-      } else if (e < nwe) {
-        const int i = e - nce;
-        const float* wr = SF(weld) + (i / 6) * WELD_WORDS;
-        x0 = wr[W_JAR + i % 6]; v = wr[W_JV + i % 6]; D = -wr[W_D + i % 6];
-      } else if (e < nedge) {
-        const float* dr = SF(dofrow) + (e - nwe) * DR_WORDS;
-        x0 = dr[DR_JAR]; v = dr[DR_JV]; D = dr[DR_D];
       }
     }
     ex[j] = x0; ev[j] = v; eD[j] = D;
   }
-  const LsVal p0 = ls_eval<HF>(c, ex, ev, eD, nedge, 0.f, g1, g2);
-  if (p0.d1 >= 0 || p0.d2 <= 0) return LsStep{0.f, 0.f};
-  gtol = fmaxf(gtol, 1e-5f * fabsf(p0.d1));  // single-precision floor on the derivative test
-  float lo = 0, hi = -1, alpha = -p0.d1 / p0.d2, best = 0, bestcost = p0.cost;
-  for (int it = 0; it < maxit; it++) {
+  // iteration -1 evaluates alpha = 0 and opens the search: one inlined copy of ls_eval serves every evaluation
+  float lo = 0, hi = -1, alpha = 0.f, best = 0, bestcost = 0.f, cost0 = 0.f;
+  ROLLED for (int it = -1; it < maxit; it++) {
     const LsVal p = ls_eval<HF>(c, ex, ev, eD, nedge, alpha, g1, g2);
+    if (it < 0) {
+      if (p.d1 >= 0 || p.d2 <= 0) return LsStep{0.f, 0.f};
+      gtol = fmaxf(gtol, 1e-5f * fabsf(p.d1));  // single-precision floor on the derivative test
+      alpha = -p.d1 / p.d2; bestcost = cost0 = p.cost;
+      continue;
+    }
     if (p.cost <= bestcost) { bestcost = p.cost; best = alpha; }
     if (fabsf(p.d1) < gtol) break;
     if (p.d1 < 0) lo = alpha; else hi = alpha;
@@ -2299,7 +2310,7 @@ HD LsStep linesearch(const Ctx c, float g1, float g2, float gtol, int maxit) {
     if (next == alpha) break;
     alpha = next;
   }
-  return LsStep{best, p0.cost - bestcost};
+  return LsStep{best, cost0 - bestcost};
 }
 
 #else
@@ -2600,7 +2611,7 @@ HD void rk4_substep(const Ctx c, bool active) {
     LANES(i, nv) { SF(rk_v0)[i] = SF(qvel)[i]; SF(rk_dx)[i] = B[0] * SF(qvel)[i]; SF(rk_df)[i] = B[0] * SF(qacc)[i]; }
     SYNC();
   }
-  for (int st = 1; st < 4; st++) {
+  ROLLED for (int st = 1; st < 4; st++) {   // one inlined copy of forward(), however small its stages are
     if (active) {
       float a = A[st - 1] * hh;
       LANES(i, nq) SF(qpos)[i] = SF(rk_q0)[i];
