@@ -46,6 +46,12 @@ class OracleAdroitHammerEnv:
         s.ctrl[:] = a                      # MujocoEnv.do_simulation
         s.step(self.frame_skip)
         obs = self._get_obs()
+        reward, goal_achieved = self.reward()
+        return obs, reward, False, False, dict(success=goal_achieved)
+
+    def reward(self):
+        """(reward, goal_achieved) of step() at the current, forwarded state."""
+        s = self.sim
         hamm_pos = s.xpos[self.obj_body_id].ravel()
         palm_pos = s.site_xpos[self.S_grasp_site_id].ravel()
         head_pos = s.site_xpos[self.tool_site_id].ravel()
@@ -65,7 +71,7 @@ class OracleAdroitHammerEnv:
                 reward += 25
             if goal_distance < 0.010:
                 reward += 75
-        return obs, reward, False, False, dict(success=goal_achieved)
+        return reward, goal_achieved
 
     def _get_obs(self):  # adroit_hammer.py:337-357
         s = self.sim
@@ -136,6 +142,12 @@ class OracleAdroitRelocateEnv(OracleAdroitHammerEnv):
         s.ctrl[:] = a
         s.step(self.frame_skip)
         obs = self._get_obs()
+        reward, goal_achieved = self.reward()
+        return obs, reward, False, False, dict(success=goal_achieved)
+
+    def reward(self):
+        """(reward, goal_achieved) of step() at the current, forwarded state."""
+        s = self.sim
         obj_pos = s.xpos[self.obj_body_id].ravel()
         palm_pos = s.site_xpos[self.S_grasp_site_id].ravel()
         target_pos = self.target_pos
@@ -152,7 +164,7 @@ class OracleAdroitRelocateEnv(OracleAdroitHammerEnv):
                 reward += 10.0
             if goal_distance < 0.05:
                 reward += 20.0
-        return obs, reward, False, False, dict(success=goal_achieved)
+        return reward, goal_achieved
 
     def _get_obs(self):  # adroit_relocate.py:331-339
         s = self.sim
@@ -216,6 +228,12 @@ class OracleAdroitPenEnv(OracleAdroitHammerEnv):
         s.ctrl[:] = a
         s.step(self.frame_skip)
         obs = self._get_obs()
+        reward, goal_achieved = self.reward()
+        return obs, reward, False, False, dict(success=goal_achieved)
+
+    def reward(self):
+        """(reward, goal_achieved) of step() at the current, forwarded state."""
+        s = self.sim
         obj_pos = s.xpos[self.obj_body_id].ravel()
         desired_loc = s.site_xpos[self.eps_ball_site_id].ravel()
         obj_orien, desired_orien = self._orien()
@@ -231,7 +249,7 @@ class OracleAdroitPenEnv(OracleAdroitHammerEnv):
                 reward += 50
             if obj_pos[2] < 0.075:
                 reward -= 5
-        return obs, reward, False, False, dict(success=goal_achieved)
+        return reward, goal_achieved
 
     def _get_obs(self):  # adroit_pen.py:339-365
         s = self.sim
@@ -289,6 +307,12 @@ class OracleAdroitDoorEnv(OracleAdroitHammerEnv):
         s.ctrl[:] = a
         s.step(self.frame_skip)
         obs = self._get_obs()
+        reward, goal_achieved = self.reward()
+        return obs, reward, False, False, dict(success=goal_achieved)
+
+    def reward(self):
+        """(reward, goal_achieved) of step() at the current, forwarded state."""
+        s = self.sim
         goal_distance = s.qpos[self.door_hinge_addrs]
         goal_achieved = goal_distance >= 1.35
         reward = 10.0 if goal_achieved else -0.1
@@ -304,7 +328,7 @@ class OracleAdroitDoorEnv(OracleAdroitHammerEnv):
                 reward += 8
             if goal_distance > 1.35:
                 reward += 10
-        return obs, reward, False, False, dict(success=goal_achieved)
+        return reward, goal_achieved
 
     def _get_obs(self):  # adroit_door.py:318-344
         s = self.sim

@@ -69,8 +69,10 @@ def lib(flavor="plain"):
         L.devsim_layout.argtypes = [vp]
         L.devsim_layout.restype = None
         L.devsim_offset.argtypes = [vp, ctypes.c_char_p, ci]
-        L.devsim_stage.argtypes = [vp, ci, ci, ci, vp]
+        L.devsim_stage.argtypes = [vp, ci, ci, ci, vp, vp]
         L.devsim_stage.restype = ci
+        L.devsim_ray_hits.argtypes = [ci, vp, ci, vp, vp, vp]
+        L.devsim_ray_hits.restype = ci
         _LIB[flavor] = L
     return _LIB[flavor]
 
@@ -88,8 +90,18 @@ def spd(nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
         raise RuntimeError(f"devsim_spd(nvp={nvp}): {L.devsim_last_error().decode()}")
 
 
-STAGE_COLLIDE, STAGE_KIN, STAGE_PROBLEM, STAGE_JV, STAGE_BUILD_H = 0, 1, 2, 3, 4
-LAYOUT = ("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE")
+def ray_hits(flavor, tp, size, p, d):
+    """ray_hits_site(tp, size, p[i], d[i]) of the `flavor` unit on the GPU for rays in the site frame: bool [n]."""
+    L = lib(flavor)
+    p, d = np.ascontiguousarray(p, np.float32), np.ascontiguousarray(d, np.float32)
+    sz, hit = np.ascontiguousarray(size, np.float32), np.zeros(len(p), np.int32)
+    if L.devsim_ray_hits(int(tp), sz.ctypes.data, len(p), p.ctypes.data, d.ctypes.data, hit.ctypes.data) != 0:
+        raise RuntimeError(f"devsim_ray_hits({flavor}): {L.devsim_last_error().decode()}")
+    return hit.astype(bool)
+
+
+STAGE_COLLIDE, STAGE_KIN, STAGE_PROBLEM, STAGE_JV, STAGE_BUILD_H, STAGE_TOUCH = 0, 1, 2, 3, 4, 5
+LAYOUT = ("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE", "C_W", "C_D", "CX_POS", "CX_PAIR", "CX_WORDS")
 
 
 class DevModel:
@@ -107,7 +119,7 @@ class DevModel:
             raise RuntimeError(f"devsim_model_create({flavor}): {L.devsim_last_error().decode()}")
         self.scr_words = L.devsim_scr_words(self._h)
         self.words = np.ctypeslib.as_array(L.devsim_model_words(self._h), shape=(L.devsim_model_nwords(self._h),)).copy()
-        lay = np.zeros(6, np.int32)
+        lay = np.zeros(len(LAYOUT), np.int32)
         L.devsim_layout(lay.ctypes.data)
         self.layout = dict(zip(LAYOUT, lay.tolist()))
 
@@ -115,6 +127,10 @@ class DevModel:
         if getattr(self, "_h", None):
             self._L.devsim_model_destroy(self._h)
             self._h = None
+
+    def model_words(self):
+        """A view of the device model words this handle uploads for every run (`words` is a copy): an edit reaches the next run."""
+        return np.ctypeslib.as_array(self._L.devsim_model_words(self._h), shape=(len(self.words),))
 
     def offset(self, name):
         o = self._L.devsim_offset(self._h, name.encode(), 0)
@@ -127,8 +143,12 @@ class DevModel:
         return o
 
     def run(self, nvp, stage, scratch):
-        """stage (STAGE_COLLIDE / STAGE_KIN / STAGE_PROBLEM / STAGE_JV / STAGE_BUILD_H) of the NVP = nvp instantiation on scratch images [n, scr_words] float32, in place."""
+        """stage (STAGE_COLLIDE / STAGE_KIN / STAGE_PROBLEM / STAGE_JV / STAGE_BUILD_H / STAGE_TOUCH) of the NVP = nvp instantiation on
+        scratch images [n, scr_words] float32, in place.  STAGE_TOUCH returns the sensor values, float32 [n, nsensor]."""
         assert scratch.dtype == np.float32 and scratch.flags.c_contiguous and scratch.shape[1] == self.scr_words
-        rc = self._L.devsim_stage(self._h, int(nvp), int(stage), scratch.shape[0], scratch.ctypes.data)
+        out = np.zeros((scratch.shape[0], self.model.nsensor), np.float32) if stage == STAGE_TOUCH else None
+        rc = self._L.devsim_stage(self._h, int(nvp), int(stage), scratch.shape[0], scratch.ctypes.data,
+                                  out.ctypes.data if out is not None else None)
         if rc != 0:
             raise RuntimeError(f"devsim_stage({self.flavor}, nvp={nvp}): {self._L.devsim_last_error().decode()}")
+        return out

@@ -20,6 +20,10 @@
 // kinematics, com_quantities, mass_matrix, collision<HF, CX>, make_constraint<HF>, smooth_forces, newton_begin<HF> (M qacc of the
 // warm start, rows_begin, the check: fcon through pass_F and grad) and build_H<HF>.  jv = rows_from_vec<HF>(c, SF(search)) on an image
 // that problem returned: with a unit vector in search it reads one column of the kernel's implicit J into the rows' JV slots.
+//
+// touch: touch_observe (touch_mode 1, the sensordata values) on an image that problem returned, or on such an image with its contact
+// records edited on the host: nsensor floats per case into `out`.  The records hold the base-row values U of the warm-start qacc that
+// newton_begin left, so the forces the sensors sum are a deterministic function of the injected state.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -123,10 +127,10 @@ done:
   return rc;
 }
 
-enum { DEVSIM_COLLIDE = 0, DEVSIM_KIN = 1, DEVSIM_PROBLEM = 2, DEVSIM_JV = 3, DEVSIM_BUILD_H = 4 };
+enum { DEVSIM_COLLIDE = 0, DEVSIM_KIN = 1, DEVSIM_PROBLEM = 2, DEVSIM_JV = 3, DEVSIM_BUILD_H = 4, DEVSIM_TOUCH = 5 };
 
 template <int NVP>
-__global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ model, int stage, float* scratch) {
+__global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ model, int stage, float* scratch, float* out) {
   const int e = blockIdx.x, lane = threadIdx.x;
   const DMHead* hg = (const DMHead*)model;
   const int hot = hg->hot_words, sw = hg->scr_words;
@@ -151,9 +155,20 @@ __global__ void __launch_bounds__(32) stage_kernel(const uint32_t* __restrict__ 
     newton_begin<HF>(c);
     build_H<HF>(c);
   } else if (stage == DEVSIM_JV) rows_from_vec<HF>(c, SF(search));
-  else build_H<HF>(c);
+  else if (stage == DEVSIM_TOUCH) {
+    FetchTask t;
+    memset(&t, 0, sizeof(t));
+    t.touch_mode = 1;
+    touch_observe(c, t, out + (size_t)e * c.h->nsensor);
+  } else build_H<HF>(c);
   __syncwarp();
   for (int k = lane; k < sw; k += 32) scratch[(size_t)e * sw + k] = s[k];
+}
+
+__global__ void ray_hits_kernel(int type, float s0, float s1, float s2, int n, const float* p, const float* d, int* hit) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const float size[3] = {s0, s1, s2};
+  if (i < n) hit[i] = ray_hits_site(type, size, p + 3 * i, d + 3 * i) ? 1 : 0;
 }
 
 #ifdef B200_WIDE
@@ -183,11 +198,16 @@ void* devsim_model_create(const void* blob, size_t n, const double* eq_data, con
   return d;
 }
 void devsim_model_destroy(void* p) { delete (DevModel*)p; }
-const uint32_t* devsim_model_words(void* p) { return ((DevModel*)p)->model.data(); }
+// the device model words, writable: devsim_stage uploads them for every run, so a test may edit a table for the runs that follow
+uint32_t* devsim_model_words(void* p) { return ((DevModel*)p)->model.data(); }
 int devsim_scr_words(void* p) { return ((const DMHead*)((DevModel*)p)->model.data())->scr_words; }
 int devsim_model_nwords(void* p) { return ((const DMHead*)((DevModel*)p)->model.data())->nwords; }
-// this library's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE
-void devsim_layout(int* out) { out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE; }
+// this library's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE, C_W, C_D, CX_POS, CX_PAIR,
+// CX_WORDS
+void devsim_layout(int* out) {
+  out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE;
+  out[6] = C_W; out[7] = C_D; out[8] = CX_POS; out[9] = CX_PAIR; out[10] = CX_WORDS;
+}
 // scratch offset of a named per-env array (DM_SCRATCH_PERSIST / DM_SCRATCH_UNION), or model offset of a model array (DM_ARRAYS)
 int devsim_offset(void* p, const char* name, int model_array) {
   const DMHead* h = (const DMHead*)((DevModel*)p)->model.data();
@@ -206,19 +226,41 @@ int devsim_offset(void* p, const char* name, int model_array) {
   return -1;
 }
 
-// run one stage (DEVSIM_COLLIDE, DEVSIM_KIN, DEVSIM_PROBLEM, DEVSIM_JV, DEVSIM_BUILD_H) of the NVP = nvp instantiation on ncase scratch images [ncase][scr_words], one block
-// each; the images are overwritten with the scratch after the stage.  Returns 0, -1 for an NVP this library does not instantiate,
-// -2 on a CUDA error.
-int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch) {
+// ray_hits_site on n rays given in the site frame: p, d [n][3] host arrays -> hit [n].  Returns 0, -2 on a CUDA error.
+int devsim_ray_hits(int type, const float* size, int n, const float* p, const float* d, int* hit) {
+  int rc = 0;
+  float *d_p = nullptr, *d_d = nullptr;
+  int* d_h = nullptr;
+  g_err[0] = 0;
+  if (n <= 0) return 0;
+  DEVSIM_OK(cudaMalloc(&d_p, sizeof(float) * 3 * n));
+  DEVSIM_OK(cudaMalloc(&d_d, sizeof(float) * 3 * n));
+  DEVSIM_OK(cudaMalloc(&d_h, sizeof(int) * n));
+  DEVSIM_OK(cudaMemcpy(d_p, p, sizeof(float) * 3 * n, cudaMemcpyHostToDevice));
+  DEVSIM_OK(cudaMemcpy(d_d, d, sizeof(float) * 3 * n, cudaMemcpyHostToDevice));
+  ray_hits_kernel<<<(n + 127) / 128, 128>>>(type, size[0], size[1], size[2], n, d_p, d_d, d_h);
+  DEVSIM_OK(cudaGetLastError());
+  DEVSIM_OK(cudaMemcpy(hit, d_h, sizeof(int) * n, cudaMemcpyDeviceToHost));
+done:
+  cudaFree(d_p); cudaFree(d_d); cudaFree(d_h);
+  return rc;
+}
+
+// run one stage (DEVSIM_COLLIDE, DEVSIM_KIN, DEVSIM_PROBLEM, DEVSIM_JV, DEVSIM_BUILD_H, DEVSIM_TOUCH) of the NVP = nvp instantiation on ncase scratch
+// images [ncase][scr_words], one block each; the images are overwritten with the scratch after the stage, and DEVSIM_TOUCH writes
+// out[ncase][nsensor] (NULL for the other stages).  Returns 0, -1 for an NVP this library does not instantiate, -2 on a CUDA error.
+int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch, float* out) {
   int rc = 0;
   const DevModel* d = (const DevModel*)p;
   const DMHead* h = (const DMHead*)d->model.data();
   uint32_t* d_m = nullptr;
-  float* d_s = nullptr;
+  float *d_s = nullptr, *d_o = nullptr;
   const size_t smem = ((size_t)h->hot_words + h->scr_words) * 4, sb = (size_t)ncase * h->scr_words * 4;
+  const size_t ob = stage == DEVSIM_TOUCH ? (size_t)ncase * h->nsensor * 4 : 0;
   g_err[0] = 0;
   DEVSIM_OK(cudaMalloc(&d_m, d->model.size() * 4));
   DEVSIM_OK(cudaMalloc(&d_s, sb));
+  if (ob) DEVSIM_OK(cudaMalloc(&d_o, ob));
   DEVSIM_OK(cudaMemcpy(d_m, d->model.data(), d->model.size() * 4, cudaMemcpyHostToDevice));
   DEVSIM_OK(cudaMemcpy(d_s, scratch, sb, cudaMemcpyHostToDevice));
   {
@@ -227,7 +269,7 @@ int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch) {
     if (nvp == V) {                                                                                                          \
       matched = 1;                                                                                                           \
       DEVSIM_OK(cudaFuncSetAttribute(stage_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
-      stage_kernel<V><<<ncase, 32, smem>>>(d_m, stage, d_s);                                                                 \
+      stage_kernel<V><<<ncase, 32, smem>>>(d_m, stage, d_s, d_o);                                                            \
     }
 #if defined(B200_WIDE)
     DEVSIM_STAGE(36)
@@ -242,8 +284,9 @@ int devsim_stage(void* p, int nvp, int stage, int ncase, float* scratch) {
   DEVSIM_OK(cudaGetLastError());
   DEVSIM_OK(cudaDeviceSynchronize());
   DEVSIM_OK(cudaMemcpy(scratch, d_s, sb, cudaMemcpyDeviceToHost));
+  if (ob) DEVSIM_OK(cudaMemcpy(out, d_o, ob, cudaMemcpyDeviceToHost));
 done:
-  cudaFree(d_m); cudaFree(d_s);
+  cudaFree(d_m); cudaFree(d_s); cudaFree(d_o);
   return rc;
 }
 }

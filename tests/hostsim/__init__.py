@@ -104,7 +104,8 @@ def lib(wide=False):
                 "hostsim_offset": (ci, [vp, ctypes.c_char_p]), "hostsim_model_offset": (ci, [vp, ctypes.c_char_p]),
                 "hostsim_forward": (None, [vp]), "hostsim_kinematics": (None, [vp]), "hostsim_step": (None, [vp, ci]),
                 "hostsim_collide": (None, [vp, ci]), "hostsim_problem": (None, [vp, ci]), "hostsim_jv": (None, [vp, ci]),
-                "hostsim_build_h": (None, [vp, ci]),
+                "hostsim_build_h": (None, [vp, ci]), "hostsim_touch": (None, [vp, vp]),
+                "hostsim_ray_hits": (None, [ci, vp, ci, vp, vp, vp]),
                 "hostsim_model": (ctypes.POINTER(ctypes.c_uint32), [vp]), "hostsim_model_words": (ci, [vp]), "hostsim_hot_words": (ci, [vp]),
                 "hostsim_layout": (None, [vp]), "hostsim_task_size": (ci, []),
                 "hostsim_env_step": (ci, [vp, vp, ci, ci] + [vp] * 7 + step_extra),
@@ -155,6 +156,14 @@ def kitchen_noise(seed, env, episode, t):
     out = np.zeros(59, dtype=np.float32)
     lib("kitchen").hostsim_kitchen_noise(int(seed) & 0xFFFFFFFFFFFFFFFF, int(env), int(episode), int(t), out.ctypes.data)
     return out
+
+
+def ray_hits(flavor, tp, size, p, d):
+    """ray_hits_site(tp, size, p[i], d[i]) of the kernel source for rays in the site frame: bool [n]."""
+    p, d = np.ascontiguousarray(p, np.float32), np.ascontiguousarray(d, np.float32)
+    sz, hit = np.ascontiguousarray(size, np.float32), np.zeros(len(p), np.int32)
+    lib(wide=flavor).hostsim_ray_hits(int(tp), sz.ctypes.data, len(p), p.ctypes.data, d.ctypes.data, hit.ctypes.data)
+    return hit.astype(bool)
 
 
 def spd(flavor, nvp, nv, A, x, dadd, hh, H, use_dadd, inplace):
@@ -231,6 +240,12 @@ class HostSim:
         """build_H<HF> alone (tests/devsim STAGE_BUILD_H)."""
         self._L.hostsim_build_h(self._h, int(nvp))
 
+    def touch(self):
+        """touch_observe with touch_mode 1 on the current scratch (tests/devsim STAGE_TOUCH): float32 [nsensor]."""
+        out = np.zeros(self.model.nsensor, np.float32)
+        self._L.hostsim_touch(self._h, out.ctypes.data)
+        return out
+
     def offset(self, name):
         o = self._L.hostsim_offset(self._h, name.encode())
         assert o >= 0, name
@@ -244,9 +259,10 @@ class HostSim:
     @property
     def layout(self):
         """This flavor's contact-record and group layout (dmodel.h enums)."""
-        lay = np.zeros(6, np.int32)
+        names = ("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE", "C_W", "C_D", "CX_POS", "CX_PAIR", "CX_WORDS")
+        lay = np.zeros(len(names), np.int32)
         self._L.hostsim_layout(lay.ctypes.data)
-        return dict(zip(("C_MU", "C_U", "C_DIMGRP", "CON_WORDS", "GRP_WORDS", "G_RANGE"), lay.tolist()))
+        return dict(zip(names, lay.tolist()))
 
     @property
     def words(self):

@@ -128,6 +128,18 @@ void hostsim_build_h(void* p, int nvp) {
   if (nvp >= 30) warp_call(base, [](const Ctx& c) { build_H<true>(c); });
   else warp_call(base, [](const Ctx& c) { build_H<false>(c); });
 }
+// touch_observe with touch_mode 1 (the sensordata values) on a scratch that hostsim_problem left, its contact records possibly edited
+// (tests/devsim STAGE_TOUCH): nsensor floats into out
+void hostsim_touch(void* p, float* out) {
+  FetchTask t;
+  memset(&t, 0, sizeof(t));
+  t.touch_mode = 1;
+  warp_call(((HostSim*)p)->ctx, [&](const Ctx& c) { touch_observe(c, t, out); });
+}
+// ray_hits_site on n rays given in the site frame: p, d [n][3] -> hit [n] (the site-frame test touch_observe runs per contact)
+void hostsim_ray_hits(int type, const float* size, int n, const float* p, const float* d, int* hit) {
+  for (int i = 0; i < n; i++) hit[i] = ray_hits_site(type, size, p + 3 * i, d + 3 * i) ? 1 : 0;
+}
 int hostsim_model_offset(void* p, const char* name) {
   const DMHead* h = ((HostSim*)p)->ctx.h;
 #define X(nm, w, kind) if (strcmp(name, #nm) == 0) return h->o_##nm;
@@ -136,8 +148,12 @@ int hostsim_model_offset(void* p, const char* name) {
   return -1;
 }
 const uint32_t* hostsim_model(void* p) { return ((HostSim*)p)->model.data(); }
-// this flavor's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE
-void hostsim_layout(int* out) { out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE; }
+// this flavor's contact-record and group layout (dmodel.h): C_MU, C_U, C_DIMGRP, CON_WORDS, GRP_WORDS, G_RANGE, C_W, C_D, CX_POS, CX_PAIR,
+// CX_WORDS
+void hostsim_layout(int* out) {
+  out[0] = C_MU; out[1] = C_U; out[2] = C_DIMGRP; out[3] = CON_WORDS; out[4] = GRP_WORDS; out[5] = G_RANGE;
+  out[6] = C_W; out[7] = C_D; out[8] = CX_POS; out[9] = CX_PAIR; out[10] = CX_WORDS;
+}
 int hostsim_task_size() { return (int)sizeof(FetchTask); }
 // one env's launch.  The kitchen flavors take `noise`, the env's observation-noise key as the step kernel builds it (NULL:
 // noise-free); the ant flavor takes `a`, the Ant's keywords as b200sim_set_ant_info leaves them with rows / origin pointing at this
